@@ -1,13 +1,13 @@
-# Convenience targets; the driver uses __graft_entry__.build(), pytest and bench.py directly.
+# Convenience targets over __graft_entry__.build(), pytest and bench.py.
 PY ?= python
 
-build:            ## libcurvine_b200.so (nvcc, sm_100a; no GPU needed) + the oracle's C restatement
+build:            ## libcurvine_b200.so (nvcc, sm_90a; no GPU needed) + the oracle's C restatement
 	$(PY) __graft_entry__.py
 
 test:             ## CPU suite (oracle, host side, stand-in runtime, kernel source on the SIMT shim)
 	$(PY) -m pytest tests -x -q -m "not gpu"
 
-test-gpu:         ## parity suite on a B200
+test-gpu:         ## parity suite on an H100
 	$(PY) -m pytest tests -x -q -m gpu
 
 sanitize:         ## host ASan/UBSan + TSan, GPU reader on the stand-in runtime (incl. stream order), kernel source on the shim

@@ -21,11 +21,10 @@ the same read over the reference's one-file-per-block mem tier through the pinne
 K2 on the GPU (`e2e_framed`), a re-read of an already-read file (`e2e_reread`), the HBM-resident K1 verify rate (`resident_verify`,
 `roofline`) and the reference's CPU reader on the host cores (`cpu_baseline`).
 Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks.  Inputs (16 GiB per GPU per
-step, never the same bytes twice) are >> L2 (126 MB): no L2 flush needed.
+step, never the same bytes twice) are >> L2 (50 MB on H100): no L2 flush needed.
 """
 import argparse
 import ctypes
-import hashlib
 import json
 import os
 import shutil
@@ -42,6 +41,7 @@ METRIC = "sequential read GB/s into HBM (CRC-verified)"
 UNIT = "GB/s"
 BLOCK = 4 << 20
 PCIE_RAW = 63.0  # PCIe Gen5 x16 per direction, GB/s (SURVEY.md 8d)
+HBM_PEAK = 3350.0  # H100 SXM HBM3 bandwidth, GB/s (data sheet)
 SEG = 256 << 20  # arena segment size
 
 
@@ -74,11 +74,15 @@ def parse():
     ap.add_argument("--dir", default="")
     ap.add_argument("--no-memory-guard", action="store_true", help="do not shrink --gib-per-gpu when the stores would not fit into the container's memory")
     ap.add_argument("--ref-materialize-gib", type=float, default=64.0, help="reference arm: how much of the file's head is written to the store (the CPU reader never reads past its sample)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write what the last headline step delivered as DIR/<name>.npy (see dump_outputs)")
+    a = ap.parse_args()
+    if a.dump_outputs and (a.impl != "ours" or a.config != "c2"):
+        ap.error("--dump-outputs writes the outputs of the headline read path only (--impl ours --config c2)")
+    return a
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -396,7 +400,7 @@ def main():
     my_blocks = shard_bytes // BLOCK
     ncpu = os.cpu_count() or 8
     threads = args.fetch_threads or max(4, min(16, ncpu // (2 * world)))
-    # loopback TCP stops scaling at ~16 connections on this box (profiles/r02_loopback_probe.txt: 46 GB/s at 16, 35 at 24, 28 at 32)
+    # loopback TCP stops scaling at ~16 connections (tools/loopback_probe.cc measures where it does on a given host)
     fthreads = args.framed_threads or max(4, min(16, ncpu // (2 * world)))
     slots = args.slots or (2 * args.verify_batch + threads + 8)
     side = args.side_steps
@@ -426,6 +430,7 @@ def main():
         head = run_leg("fresh", cluster, fs, args.tier, args, rank, world, dist, dst, shard_bytes, args.steps, args.warmup, True, 5000)
         launches = (K.launch_count() - launches0) * args.steps // max(1, args.steps + args.warmup)
         arena1 = fs.arena_stats()
+        dumped = dump_outputs(args, dst, shard_bytes, head, world) if args.dump_outputs else None  # before the side legs overwrite dst
         # ---- side legs
         legs = set(x for x in args.legs.split(",") if x) if side > 0 else set()
         if world > 1:  # beyond one GPU the side legs are the re-read and the kernel-only pass; the transport legs are one-GPU numbers
@@ -524,12 +529,7 @@ def main():
         per_step_e2e = [maxr(x) for x in head["e2e_ms"]]
 
         if rank == 0:
-            peaks = {}
-            try:
-                peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-            except Exception:
-                pass
-            hbm_peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)") if "hbm_gbs" in peaks else (6650.0, "fallback (B200_PROFILING.md)")
+            hbm_peak, peak_src = HBM_PEAK, "NVIDIA H100 SXM data sheet (HBM3, 700 W card)"
             gbps = lambda ms: n_total / ms / 1e6 if ms else None
             e2e_val, ing_val = gbps(e2e_ms), gbps(ing_ms)
             stats = head["stats"]
@@ -561,8 +561,8 @@ def main():
                 "gpu_launches": int(launches),
                 "resident_verify": {"value": gbps(res_ms), "unit": UNIT, "ms": res_ms, "what": "K1 + fold over the bytes already in HBM (no ingest): an HBM-bound kernel rate, not a read rate"},
                 "roofline": {"bound": "hbm", "kernel": "walk_kernel<CRC,!DST> (K1 CRC verify)", "achieved": shard_bytes / walk_avg_ms / 1e6, "peak": hbm_peak,
-                             "unit": "GB/s", "frac": shard_bytes / walk_avg_ms / 1e6 / hbm_peak, "traffic": ncu_traffic(shard_bytes), "peak_source": peak_src,
-                             "note": "K1 only reads (N bytes in, 4 bytes per block out) while the peak is a read+write copy rate, so frac can exceed 1. The metric itself "
+                             "unit": "GB/s", "frac": shard_bytes / walk_avg_ms / 1e6 / hbm_peak, "peak_source": peak_src,
+                             "note": "K1 only reads (N bytes in, 4 bytes per block out); the peak is the data sheet's, not a rate measured on this card. The metric itself "
                                      "is bound by PCIe ingest (e2e.frac_of_pcie_gen5_x16_raw_63GBps), under which K1 hides completely.",
                              "algorithmic_bytes_per_launch": shard_bytes, "avg_launch_ms": walk_avg_ms, "launches_timed": int(walk_n.value)},
                 "clocks": sampler.summary(head["windows"]),
@@ -591,6 +591,12 @@ def main():
     finally:
         sampler.stop()
         cluster.close()
+    if dumped is not None:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        suffix = "" if world == 1 else "_rank%d" % rank
+        for name, arr in dumped.items():
+            np.save(os.path.join(args.dump_outputs, name + suffix + ".npy"), arr)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()
@@ -598,17 +604,35 @@ def main():
         emit(out)
 
 
-def ncu_traffic(shard_bytes):
-    """dram bytes per K1 launch from the committed `ncu --set full` capture -- only when that capture was taken from THIS kernels.cu
-    at this launch size; anything else reports null rather than a stale constant."""
-    try:
-        rec = json.load(open(os.path.join(ROOT, "profiles", "k1_ncu_traffic.json")))
-        sha = hashlib.sha256(open(os.path.join(ROOT, "curvine_b200", "csrc", "kernels.cu"), "rb").read()).hexdigest()
-        if rec.get("kernels_cu_sha256") == sha and rec.get("launch_bytes") == shard_bytes:
-            return rec.get("dram_bytes_per_launch")
-    except Exception:
-        pass
-    return None
+DUMP_SAMPLE = 4 << 20  # bytes of the delivered buffers sampled into dst_sample*.npy over all ranks (~48 MiB with their positions)
+
+
+def dump_outputs(args, dst, shard_bytes, head, world):
+    """What a caller of the headline path holds after its last timed step, as float64/float32 arrays (integers below 2^53 are exact):
+      dst_sample      the bytes cv_read_device left in HBM at DUMP_SAMPLE / world fixed positions (seeded, sorted; first and last byte included)
+      dst_sample_pos  those positions
+      block_crc       CRC of every block of that buffer, recomputed by K1 (cvk_crc_blocks) over the bytes in HBM
+      verify          cv_verify's answer: [sum of the block CRCs, mismatching blocks, verified blocks], and the bytes read
+    The step's file is synthetic and seeded by its inode, so the same arguments give the same inputs on every run."""
+    import numpy as np
+    import torch
+    from curvine_b200 import _lib
+    n_blocks = shard_bytes // BLOCK
+    pos = np.random.RandomState(20261015).randint(0, shard_bytes, size=min(DUMP_SAMPLE // world, shard_bytes), dtype=np.int64)
+    pos[0], pos[-1] = 0, shard_bytes - 1
+    pos.sort()
+    sample = dst[torch.from_numpy(pos).to(dst.device)].cpu().numpy()
+    d_off = torch.arange(n_blocks, dtype=torch.int64, device=dst.device) * BLOCK
+    d_len = torch.full((n_blocks,), BLOCK, dtype=torch.int64, device=dst.device)
+    d_crc = torch.empty(n_blocks, dtype=torch.int32, device=dst.device)
+    _lib.check(_lib.lib().cvk_crc_blocks(ctypes.c_void_p(dst.data_ptr()), ctypes.c_void_p(d_off.data_ptr()), ctypes.c_void_p(d_len.data_ptr()), n_blocks,
+                                         args.poly, shard_bytes, ctypes.c_void_p(d_crc.data_ptr()), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)),
+               "cvk_crc_blocks")
+    torch.cuda.synchronize()
+    crc = d_crc.cpu().numpy().view(np.uint32)
+    assert int(crc.astype(np.uint64).sum()) == head["sum_crc"], "K1 over the delivered bytes disagrees with cv_verify"
+    return {"dst_sample": sample.astype(np.float32), "dst_sample_pos": pos.astype(np.float64), "block_crc": crc.astype(np.float64),
+            "verify": np.array([head["sum_crc"], 0, n_blocks, shard_bytes], dtype=np.float64)}
 
 
 # ------------------------------------------------------------------ the reference's CPU read path (oracle port)

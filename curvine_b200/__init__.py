@@ -1,4 +1,4 @@
-"""curvine_b200: B200-native sequential block-read path for Curvine (see DESIGN.md).
+"""curvine_b200: GPU-native (H100, sm_90a) sequential block-read path for Curvine (see DESIGN.md).
 
 The package is a thin Python mirror over libcurvine_b200.so's C ABI (include/*.h);
 importing it never falls back to a CPU implementation.

@@ -11,9 +11,8 @@
 // client maps and pins the segments once, at mount time, off the read path; after that EVERY block the worker ever
 // stores there -- including files written later -- is DMA-able at once: there is no per-file or per-block client state,
 // so a never-read file streams at the same rate as a re-read.  The worker serves framed reads by sendfile(2) out of the
-// segment file (measured on the B200 box, profiles/r02_loopback_probe.txt: 46 GB/s over 16 loopback TCP connections out of one
-// large tmpfs file, against 24 GB/s for send(2) from a mapping of it -- the copy into socket buffers costs more than the page
-// references sendfile takes).
+// segment file (tools/loopback_probe.cc compares it with send(2) from a mapping of the segment: the copy into socket buffers
+// costs more than the page references sendfile takes).
 //
 // On-disk state (survives a worker restart like the reference's block files do): the reference path
 // <base>/active/bX/bY/blk_<id> holds a one-line extent descriptor "CVARENA1 <seg> <off> <len>\n" instead of the bytes;

@@ -410,7 +410,7 @@ int64_t cv_device_stats(cv_reader* r, CvReadStats* out) {
 int64_t cv_gds_info(int64_t out[2]) {
     API_NEED(out);
     const GdsInfo& g = gds_info();
-    out[0] = g.available, out[1] = g.compat;
+    out[0] = g.available, out[1] = 0;  // out[1]: reserved (cuFile's compatibility mode is never used)
     g_last_error = g.detail;
     const std::string why = gds_last_refusal();
     if (!why.empty()) g_last_error += "; first refusal: " + why;

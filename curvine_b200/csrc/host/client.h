@@ -1,7 +1,7 @@
 // Client reader stack (host side): namespace lookup, block RPC client + pool, block readers with replica
 // failover, and the file-level reader that implements the reference `Reader` trait semantics.
 //
-// Mirrors (reference, relative to /root/reference):
+// Mirrors (reference, relative to the CurvineIO/curvine source tree):
 //   curvine-common/src/state/block_info.rs:66-72,127-131,156-217   ExtendedBlock / LocatedBlock / FileBlocks / search
 //   curvine-client/src/block/block_client.rs:222-300               open_block / read_data / read_commit
 //   orpc/src/client/raw_client.rs:100-116                          req_id/seq_id echo check

@@ -65,8 +65,8 @@ struct B200Conf {
     bool local_unix_socket = false;  // block connections to a worker on this host use its abstract unix socket (net.h) instead of loopback TCP
     int64_t socket_buffer = 0;       // explicit SO_RCVBUF/SO_SNDBUF for block connections (0 = kernel autotuning)
     int gds = 2;                  // "gds" = "off" | "on" | "auto": short-circuit reads of SSD/HDD/DISK-tier blocks go through cuFileRead
-                                  // (gds.h) straight into HBM; auto (default) = only with real GPUDirect Storage (nvidia-fs), on = also in
-                                  // cuFile's compatibility mode; anything GDS cannot serve goes through the pinned ring
+                                  // (gds.h) straight into HBM where the host has GPUDirect Storage (nvidia-fs); "on" and "auto" (default)
+                                  // are the same (cuFile's compatibility mode is never used); anything GDS cannot serve takes the pinned ring
     int numa_node = -1;           // bind fetch threads to this node's CPUs (-1: the GPU's node if discoverable, -2: no binding)
 };
 

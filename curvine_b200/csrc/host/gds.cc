@@ -54,6 +54,13 @@ std::unordered_map<std::string, Entry> g_files;
 std::string g_refusal;  // first reason a file was turned away (under g_mu)
 
 void probe() {
+    // Without the nvidia-fs kernel module cuFile can only run its POSIX compatibility mode, and its driver open can block
+    // indefinitely there (observed on H100 hosts without nvidia-fs: cuFileDriverOpen never returned).  GDS is reported
+    // unavailable instead and every disk-tier block takes the pinned ring.
+    if (access("/proc/driver/nvidia-fs/stats", R_OK) != 0) {  // the nvidia-fs module publishes this file
+        g_info.detail = "nvidia-fs kernel module not loaded: no GPUDirect Storage";
+        return;
+    }
     const char* names[] = {"libcufile.so.0", "libcufile.so", "/usr/local/cuda/lib64/libcufile.so.0", "/usr/local/cuda/lib64/libcufile.so"};
     for (const char* n : names)
         if ((g_api.lib = dlopen(n, RTLD_NOW | RTLD_LOCAL))) break;
@@ -75,8 +82,7 @@ void probe() {
         return;
     }
     g_info.available = true;
-    g_info.compat = access("/proc/driver/nvidia-fs/stats", R_OK) != 0;  // the nvidia-fs module publishes this file
-    g_info.detail = g_info.compat ? "cuFile compatibility mode (nvidia-fs kernel module not loaded)" : "GPUDirect Storage (nvidia-fs)";
+    g_info.detail = "GPUDirect Storage (nvidia-fs)";
 }
 
 }  // namespace
@@ -120,9 +126,8 @@ Err gds_read(const std::string& path, void* d_dst, int64_t n, int64_t file_off) 
         }
         if (it == g_files.end()) {
             Entry ne;
-            // real GDS wants O_DIRECT; the compatibility mode does plain preads at whatever offset the caller asks for, which an
-            // O_DIRECT descriptor would refuse unless 512-byte aligned
-            ne.fd = g_info.compat ? -1 : ::open(path.c_str(), O_RDONLY | O_DIRECT | O_CLOEXEC);
+            // GDS wants O_DIRECT; a file system that refuses it gets a plain descriptor (cuFileHandleRegister then decides)
+            ne.fd = ::open(path.c_str(), O_RDONLY | O_DIRECT | O_CLOEXEC);
             if (ne.fd < 0) ne.fd = ::open(path.c_str(), O_RDONLY | O_CLOEXEC);
             if (ne.fd < 0) return Err::io(str_printf("open %s: %s", path.c_str(), strerror(errno)));
             CvCuFileDescr d;

@@ -1,16 +1,15 @@
 // GPUDirect Storage for the SSD/HDD tiers (SURVEY.md 8f-2): cuFileRead straight into the destination in HBM, no pinned host
 // ring in between.  libcufile is dlopen'ed at first use (the product library carries no link-time dependency on it); when it is
 // missing, when the driver cannot be opened, or when a file cannot be registered, the caller falls back to the pinned ring and
-// says so in the read stats.  Without the nvidia-fs kernel module cuFile runs in its compatibility mode (POSIX reads into its own
-// pinned bounce buffers + copies): functional, and reported as such (GdsInfo::compat).
+// says so in the read stats.  Without the nvidia-fs kernel module GDS is reported unavailable and cuFile is never opened: it could
+// only run its compatibility mode (POSIX reads into its own bounce buffers + copies), whose driver open can block indefinitely.
 #pragma once
 #include "common.h"
 
 namespace cv {
 
 struct GdsInfo {
-    bool available = false;  // libcufile loaded and cuFileDriverOpen succeeded
-    bool compat = false;     // no nvidia-fs: cuFile's POSIX compatibility mode
+    bool available = false;  // nvidia-fs loaded, libcufile loaded and cuFileDriverOpen succeeded
     std::string detail;
 };
 

@@ -198,7 +198,7 @@ static bool stat_stamps(const std::vector<std::string>& paths, std::vector<uint6
 
 // Background registration: a cache miss does not stall the read.  The foreground moves the group through the pinned
 // ring right away (cold pass at ring speed) while a few registrar threads mmap + cudaHostRegister the same files so that
-// the NEXT pass over them is zero-copy.  cudaHostRegister pins 4 KiB pages at ~13-26 GB/s on the B200 box and
+// the NEXT pass over them is zero-copy.  cudaHostRegister pins 4 KiB pages at a few GB/s per thread and
 // serialises with copy enqueues inside the driver, so by default (`register_when_idle`) the registrar threads yield to
 // reads in flight: `hold` counts them, and a registrar only starts a new group while it is zero (or while a caller is
 // blocked in drain()).
@@ -1117,7 +1117,9 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
         for (size_t j = g * k; j < std::min(J, g * k + k); j++) group_verbatim[g] |= mode[j] == kFramed;
     std::vector<int64_t> req_ids(J, 0);
     std::atomic<bool> use_mapped{bc.zero_copy};
-    std::atomic<bool> use_gds{!call_framed && bc.gds != 0 && gds_info().available && (bc.gds == 1 || !gds_info().compat)};
+    bool any_disk = false;  // cuFile is probed only by a read that has disk-tier blocks
+    for (size_t j = 0; j < J && !any_disk; j++) any_disk = (*jobs[j].lb).block.storage_type != kStorageMem;
+    std::atomic<bool> use_gds{!call_framed && bc.gds != 0 && any_disk && gds_info().available};
     std::atomic<uint64_t> gds_bytes{0};
     std::mutex held_mu;
     const int T_threads = static_cast<int>(std::min<size_t>(static_cast<size_t>(std::max(1, bc.fetch_threads)), NG));

@@ -11,10 +11,10 @@ namespace cv {
 // timer becomes io::ErrorKind::TimedOut, i.e. FsError::IO, orpc/src/io/io_error.rs:148-153)
 Err tcp_connect(const std::string& host, int port, int* fd_out, int64_t conn_timeout_ms = 0, int64_t io_timeout_ms = 0);
 Err tcp_listen(const std::string& host, int port, int* fd_out, int* bound_port);
-// Same-host transport beside TCP (B200-side addition, no reference counterpart): the worker also listens on the ABSTRACT unix socket
+// Same-host transport beside TCP (an addition of this project, no reference counterpart): the worker also listens on the ABSTRACT unix socket
 // "curvine-b200-worker-<tcp port>" (no file system entry, same network namespace as the loopback port); a local client that is
-// configured for it ([b200] local_unix_socket) connects there first.  Same frames, same handlers -- measured on the B200 box
-// (profiles/r02_loopback_probe.txt): 54.6 GB/s over 16 unix connections against 46.5 GB/s over 16 loopback TCP connections.
+// configured for it ([b200] local_unix_socket) connects there first.  Same frames, same handlers; unix
+// sockets with sendfile carry more than loopback TCP at the same connection count (tools/loopback_probe.cc measures both).
 std::string local_socket_name(int tcp_port);
 Err unix_listen(const std::string& abstract_name, int* fd_out);
 Err unix_connect(const std::string& abstract_name, int* fd_out, int64_t io_timeout_ms = 0);

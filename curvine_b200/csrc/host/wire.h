@@ -1,6 +1,6 @@
 // orpc RpcMessage frame codec + the protobuf headers on the block-read path.
 //
-// Mirrors (reference, relative to /root/reference):
+// Mirrors (reference, relative to the CurvineIO/curvine source tree):
 //   orpc/src/message/rpc_message.rs:26-41,43-90,301-338   Protocol / Status / encode_protocol / decode_protocol
 //   orpc/src/handler/rpc_frame.rs:205-264                  Frame::send / Frame::receive (heartbeats skipped)
 //   orpc/src/error/error_encoder.rs:24-51                  error body layout

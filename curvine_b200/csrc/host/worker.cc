@@ -2,6 +2,8 @@
 
 #include <errno.h>
 #include <fcntl.h>
+#include <poll.h>
+#include <sys/eventfd.h>
 #include <sys/socket.h>
 #include <sys/stat.h>
 #include <sys/vfs.h>
@@ -317,24 +319,41 @@ Err Worker::start(const std::vector<std::string>& data_dirs, const std::string& 
                   const ArenaOpts& arena) {
     CV_RETURN_IF_ERR(store_.init(data_dirs, cluster_id, arena));
     enable_send_file_ = enable_send_file;
-    CV_RETURN_IF_ERR(tcp_listen(host, port, &listen_fd_, &port_));
+    wake_fd_ = eventfd(0, EFD_CLOEXEC);
+    if (wake_fd_ < 0) return Err::io(str_printf("eventfd: %s", strerror(errno)));
+    if (Err e = tcp_listen(host, port, &listen_fd_, &port_)) {
+        close_fd(wake_fd_);
+        wake_fd_ = -1;
+        return e;
+    }
+    // non-blocking listeners: a connection reset between poll() and accept() must not leave accept() blocked where stop() cannot reach it
+    fcntl(listen_fd_, F_SETFL, fcntl(listen_fd_, F_GETFL) | O_NONBLOCK);
     stopping_ = false;
     accept_thread_ = std::thread([this] { accept_loop(listen_fd_); });
-    if (!unix_listen(local_socket_name(port_), &unix_fd_)) unix_accept_thread_ = std::thread([this] { accept_loop(unix_fd_); });
-    else unix_fd_ = -1;  // no same-host transport (name taken): TCP serves everyone
+    if (!unix_listen(local_socket_name(port_), &unix_fd_)) {
+        fcntl(unix_fd_, F_SETFL, fcntl(unix_fd_, F_GETFL) | O_NONBLOCK);
+        unix_accept_thread_ = std::thread([this] { accept_loop(unix_fd_); });
+    } else {
+        unix_fd_ = -1;  // no same-host transport (name taken): TCP serves everyone
+    }
     return Err::ok();
 }
 
 void Worker::stop() {
     if (listen_fd_ < 0) return;
     stopping_ = true;
-    ::shutdown(listen_fd_, SHUT_RDWR);  // wakes accept(); the descriptor stays valid (and ours) until the accept thread is gone
+    // the eventfd wakes both accept loops' poll(); shutdown() of a listening socket alone does not wake a waiter on every kernel / sandbox
+    const uint64_t one = 1;
+    const ssize_t w = ::write(wake_fd_, &one, sizeof(one));  // fails only on a full counter, which is readable anyway
+    (void)w;
+    ::shutdown(listen_fd_, SHUT_RDWR);
     if (unix_fd_ >= 0) ::shutdown(unix_fd_, SHUT_RDWR);
     if (accept_thread_.joinable()) accept_thread_.join();
     if (unix_accept_thread_.joinable()) unix_accept_thread_.join();
     close_fd(listen_fd_);
     close_fd(unix_fd_);
-    listen_fd_ = unix_fd_ = -1;
+    close_fd(wake_fd_);
+    listen_fd_ = unix_fd_ = wake_fd_ = -1;
     {
         std::lock_guard<std::mutex> lk(conn_mu_);
         for (int fd : conn_fds_) ::shutdown(fd, SHUT_RDWR);
@@ -344,9 +363,16 @@ void Worker::stop() {
 
 void Worker::accept_loop(int lfd) {
     while (!stopping_) {
-        const int fd = ::accept(lfd, nullptr, nullptr);
-        if (fd < 0) {
+        pollfd p[2] = {{lfd, POLLIN, 0}, {wake_fd_, POLLIN, 0}};
+        if (::poll(p, 2, -1) < 0) {
             if (errno == EINTR) continue;
+            break;
+        }
+        if (p[1].revents) break;  // stop()
+        if (!(p[0].revents & POLLIN)) break;  // the listening socket failed
+        const int fd = ::accept4(lfd, nullptr, nullptr, 0);  // blocking connection socket: accept4 does not pass O_NONBLOCK on
+        if (fd < 0) {
+            if (errno == EINTR || errno == EAGAIN || errno == EWOULDBLOCK || errno == ECONNABORTED) continue;  // reset or taken meanwhile
             break;
         }
         set_sock_opts(fd);

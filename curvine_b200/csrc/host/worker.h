@@ -123,6 +123,7 @@ class Worker {
     HbmTier hbm_;
     WorkerMetrics metrics_;
     int listen_fd_ = -1, unix_fd_ = -1;  // TCP, and the same-host abstract unix socket named after the TCP port (net.h)
+    int wake_fd_ = -1;  // eventfd that stop() signals; the accept loops poll it beside their listening socket
     std::thread unix_accept_thread_;
     int port_ = 0;
     bool enable_send_file_ = true;

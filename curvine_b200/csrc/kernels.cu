@@ -1,4 +1,4 @@
-// sm_100a kernels for the Curvine sequential block-read path + their extern "C" launchers
+// sm_90a kernels for the Curvine sequential block-read path + their extern "C" launchers
 // (declared in include/curvine_b200_kernels.h, which cites the reference code each one replaces).
 //
 // This is a byte-stream / integer path: no tensor cores.  Design (see DESIGN.md §3):
@@ -13,7 +13,7 @@
 //   * The same row walker optionally stores the (re-aligned) vectors to a destination, which gives the
 //     fused frame-unpack+gather+CRC (K2), frame-pack+CRC (K4) and page scatter/gather (K3) kernels.
 // Launch train of one call: prep_* (piece geometry) -> scan_counts (prefix sum of per-piece unit counts) -> expand_units
-// (one 32-byte record per unit) -> walk_kernel (persistent: one 1024-thread CTA per SM, 148 on B200, contiguous unit range per
+// (one 32-byte record per unit) -> walk_kernel (persistent: one 1024-thread CTA per SM, 132 on H100 SXM, contiguous unit range per
 // CTA, a warp per unit) -> fold_blocks (unit partials -> one CRC per block).  Workspaces come from a private memory pool.
 #include <cuda_runtime.h>
 
@@ -915,7 +915,7 @@ __global__ void verify_crcs_kernel(const uint32_t* crc, const uint32_t* expect, 
 // ------------------------------------------------------------------ host side
 
 static std::atomic<uint64_t> g_launches{0};
-// Tuning of the DST walkers (cvk_tune; defaults chosen from the kbench sweeps in profiles/): rows per tile, and
+// Tuning of the DST walkers (cvk_tune; defaults chosen from tools/kbench.py sweeps): rows per tile, and
 // register-tiled vs shared-memory staged walks.  (An L1::no_allocate load flavour was swept too: no gain, removed.)
 static std::atomic<int> g_tile_crc_dst{4}, g_tile_copy{2};
 static std::atomic<bool> g_staged{false};  // cvk_tune(3, 1) / CVK_STAGED=1: shared-memory staged (cp.async) DST walks for local sources

@@ -2,7 +2,7 @@
  * curvine_b200.h -- upper boundary: the reader surface a Curvine client binds to (C ABI).
  *
  * Drop-in for the reference's reader path only.  Semantics, ownership, error and threading conventions are
- * the reference's own FFI conventions (curvine-libsdk, paths relative to /root/reference):
+ * the reference's own FFI conventions (curvine-libsdk, paths relative to the CurvineIO/curvine source tree):
  *   handles      opaque pointers (Box::into_raw as i64: orpc/src/sys/ffi_utils.rs:47-49,64-66)
  *   errors       0 == SUCCESS (curvine-libsdk/src/java/mod.rs:23); failure returns -(ErrorKind)
  *                (curvine-common/src/error/fs_error.rs:35-66,324-326); EOF is not an error (length 0)
@@ -137,8 +137,8 @@ typedef struct CvReadStats {
     uint64_t reg_bytes;            /* bytes registered through the cache right now (<= register_cache) */
     uint64_t gds_bytes;            /* bytes read file -> HBM by cuFileRead (disk tiers, [b200] gds) */
 } CvReadStats;
-/* GPUDirect Storage probe: out[0] = 1 when libcufile loaded and its driver opened, out[1] = 1 when it runs in compatibility
- * mode (no nvidia-fs kernel module).  The message (cv_last_error) carries the detail either way. */
+/* GPUDirect Storage probe: out[0] = 1 when the nvidia-fs kernel module is loaded and libcufile loaded and its driver opened;
+ * out[1] is reserved and always 0 (cuFile's compatibility mode is never used).  The message (cv_last_error) carries the detail. */
 int64_t cv_gds_info(int64_t out[2]);
 int64_t cv_device_stats(cv_reader* r, CvReadStats* out);
 

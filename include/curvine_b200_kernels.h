@@ -1,5 +1,5 @@
 /*
- * curvine_b200_kernels.h -- lower boundary: host -> CUDA (sm_100a) launchers.
+ * curvine_b200_kernels.h -- lower boundary: host -> CUDA (sm_90a) launchers.
  *
  * The "thin extern C layer" the north_star asks for (SURVEY.md §8b, lower boundary):
  * plain launchers, no C++ or torch types in signatures, the caller owns all memory,
@@ -7,7 +7,7 @@
  * cudaError_t as int (0 == cudaSuccess) and never throws or aborts.  A Rust host binds
  * these with an `extern "C"` block 1:1 (see INTEGRATION.md).
  *
- * What each launcher replaces in the reference (paths relative to /root/reference):
+ * What each launcher replaces in the reference (paths relative to the CurvineIO/curvine source tree):
  *   cvk_crc_blocks      Utils::crc32 on the caller thread   orpc/src/common/utils.rs:73-75,
  *                       as used per read buffer by          curvine-tests/src/curvine_bench.rs:37-48,222-231
  *   cvk_unpack_frames   RpcFrame::receive + decode_protocol orpc/src/handler/rpc_frame.rs:222-264,

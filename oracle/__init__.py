@@ -8,10 +8,9 @@ reader beside the GPU path exactly as bench.py's CPU-baseline leg does), and the
 only as the checker (or as the timed CPU baseline), never as the thing shipped.
 
 It is a *restatement* of the reference's algorithm for this path, written from
-the reference sources cited function by function (paths relative to
-``/root/reference``).  The reference is Rust and cannot be built in this image
-(no cargo/rustc, no network, crates not vendored), so there is no
-``oracle/_ref``.
+the reference sources cited function by function (paths relative to the
+CurvineIO/curvine source tree).  The reference is Rust (905 crates, not
+vendored), so no binary of it is built beside the oracle.
 
 Pinning status (SURVEY.md §8c):
   * wire status byte  -- pinned by the reference's only known-answer test,

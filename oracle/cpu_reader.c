@@ -5,7 +5,7 @@
  * The reference is Rust and cannot be built in this image; this port is what bench.py times as
  * cpu_baseline (kind "port") and as the `--impl reference` arm.
  *
- * Structure followed (paths relative to /root/reference):
+ * Structure followed (paths relative to the CurvineIO/curvine source tree):
  *   caller loop     read_full(128 KiB buf) + Utils::crc32(buf) on the caller thread, u64 sum
  *                   curvine-tests/src/curvine_bench.rs:212-236,37-48
  *   Reader::read    one memcpy per byte out of the current chunk       curvine-common/src/fs/reader.rs:71-81

@@ -5,7 +5,7 @@
  * bench.py's cpu_baseline / --impl reference legs as the checker or the timed CPU baseline; never
  * linked into or called by the product (curvine_b200/).
  *
- * What it restates (paths relative to /root/reference):
+ * What it restates (paths relative to the CurvineIO/curvine source tree):
  *   cvo_crc32 / cvo_crc32c      Utils::crc32 = crc32fast::hash        orpc/src/common/utils.rs:73-75
  *                               (crc32fast 1.4.2/1.5.0 is a crates.io dependency, absent from the tree:
  *                               restated from the published CRC-32/ISO-HDLC definition; pinned to the

@@ -2,7 +2,7 @@
 
 Oracle / test infrastructure only (see oracle/__init__.py).
 
-Follows (reference, relative to /root/reference):
+Follows (reference, relative to the CurvineIO/curvine source tree):
   * curvine-common/src/fs/reader.rs:50-141          read_chunk / read / read_full / fuse_read
   * curvine-client/src/file/fs_reader.rs:103-126     read_chunk0, seek fast path inside the chunk
   * curvine-client/src/file/fs_reader_buffer.rs:248-323  sub-reader choice, misaligned-chunk trim

@@ -3,7 +3,7 @@
  *
  * TEST INFRASTRUCTURE / CPU BASELINE ONLY (see oracle/__init__.py).  Never linked into the product; it exists so
  * that `bench.py --impl reference` times the oracle's CPU reader (cpu_reader.c) against something that is NOT the
- * product library.  It restates the worker side of the block-read path (paths relative to /root/reference):
+ * product library.  It restates the worker side of the block-read path (paths relative to the CurvineIO/curvine source tree):
  *   BlockStore layout   <base>/active/b{(id>>48)&31}/b{(id>>32)&31}/blk_<id>, raw bytes
  *                       curvine-server/src/worker/block/block_meta.rs:199-237
  *   server loop         one stateful handler per connection, request -> handle -> response; errors become error responses

@@ -2,7 +2,7 @@
 
 Oracle / test infrastructure only (see oracle/__init__.py).
 
-Follows (reference, relative to /root/reference):
+Follows (reference, relative to the CurvineIO/curvine source tree):
   * orpc/src/message/rpc_message.rs:26-41   PROTOCOL_SIZE=22, HEAD_SIZE=18, MAX_DATE_SIZE=16 MiB
   * orpc/src/message/rpc_message.rs:43-90   RequestStatus / ResponseStatus / Status::{encode,from}
   * orpc/src/message/rpc_message.rs:301-338 encode_protocol / decode_protocol (big-endian)

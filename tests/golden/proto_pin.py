@@ -3,7 +3,7 @@ in the image).  Test infrastructure: pins the byte-level restatements in oracle/
 against a third implementation of the protobuf wire format, so that the header bytes are no longer checked only against
 themselves (VERDICT r1: "frame/protobuf bytes: parity unpinned").
 
-The message shapes are restated from the reference's .proto files, field by field (paths relative to /root/reference):
+The message shapes are restated from the reference's .proto files, field by field (paths relative to the CurvineIO/curvine source tree):
     curvine-common/proto/worker.proto:10-18   BlockWriteRequest
     curvine-common/proto/worker.proto:27-34   BlockWriteResponse       (pipeline_status, field 6, is not on this path: omitted)
     curvine-common/proto/worker.proto:38-47   BlockReadRequest

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY -- plain-loop CPU stand-ins for the cvk_* launchers (include/curvine_b200_kernels.h), linked
 // into the mock library instead of csrc/kernels.cu so the host pipeline above them can run without a GPU.  They restate
 // the launchers' CONTRACT (what lands where, which flags are raised), not the kernels' algorithm: a bytewise table CRC, memcpy.
-// The real kernels are checked against the oracle on a B200 by tests/test_kernels_gpu.py; nothing here is ever timed or shipped.
+// The real kernels are checked against the oracle on an H100 by tests/test_kernels_gpu.py; nothing here is ever timed or shipped.
 #include <string.h>
 
 #include <atomic>

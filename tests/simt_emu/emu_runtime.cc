@@ -7,8 +7,8 @@
 extern "C" {
 cudaError_t cudaDeviceGetAttribute(int* value, enum cudaDeviceAttr attr, int) {
     if (attr != cudaDevAttrMultiProcessorCount) return cudaErrorInvalidValue;
-    const char* e = getenv("CV_SIMT_EMU_SMS");  // persistent kernels launch one CTA per SM: 148 on the B200
-    *value = e ? atoi(e) : 148;
+    const char* e = getenv("CV_SIMT_EMU_SMS");  // persistent kernels launch one CTA per SM: 132 on the H100 SXM
+    *value = e ? atoi(e) : 132;
     return cudaSuccess;
 }
 cudaError_t cudaMemPoolCreate(cudaMemPool_t* pool, const struct cudaMemPoolProps*) {

@@ -78,7 +78,7 @@ namespace cv_emu {
 namespace {
 
 constexpr size_t kStackBytes = 64 << 10;
-constexpr size_t kDynSmemBytes = 232448;  // 227 KB, the per-CTA maximum on sm_100
+constexpr size_t kDynSmemBytes = 232448;  // 227 KB, the per-CTA maximum on sm_90
 constexpr unsigned kMaxThreads = 1024;
 
 enum State : uint8_t { kRunnable, kWaitWarp, kWaitBlock, kDone };

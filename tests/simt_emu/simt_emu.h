@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY -- a SIMT execution shim that lets g++ compile csrc/kernels.cu (the product's kernel source, unmodified
 // apart from the mechanical launch/asm rewrite of tests/simt_emu/build.py) and run its __global__ functions on host cores, so the
-// kernels' ALGORITHM is checked against the oracle by the CPU suite too (the GPU suite checks the compiled sm_100a code on a B200).
+// kernels' ALGORITHM is checked against the oracle by the CPU suite too (the GPU suite checks the compiled sm_90a code on an H100).
 //
 // Execution model: one fiber per CUDA thread, one thread block at a time per host worker thread, blocks of a grid spread over the
 // workers.  A fiber runs until it reaches a collective (__syncthreads, __syncwarp, a *_sync warp intrinsic) or returns; collectives

@@ -35,7 +35,7 @@ def _shim_env():
     return dict(os.environ, CV_TEST_MOCK_CUDA_LIB=mod.build(), MOCK_CUDA_ASYNC="1", MOCK_CUDA_JITTER_US="300", CV_SIMT_EMU_THREADS="4")
 
 
-def test_own_arm_control_flow_and_json_line_on_the_mock_runtime():
+def test_own_arm_control_flow_and_json_line_on_the_mock_runtime(tmp_path):
     """bench.py's own arm (arena mount, context warm-up read, fresh-file steps, re-read / pread / framed side legs, HBM-resident K1
     steps, roofline, cpu_baseline) executed end to end without a GPU: tests/mock_cuda/run_bench_on_mock.py swaps in the mock library and
     tells torch that "cuda" tensors are CPU tensors.  Checks the control flow and the contract of the printed line; every number
@@ -43,7 +43,7 @@ def test_own_arm_control_flow_and_json_line_on_the_mock_runtime():
     env = _shim_env()
     gib, steps, warmup = 0.25, 2, 2
     p = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "mock_cuda", "run_bench_on_mock.py"), "--gib-per-gpu", str(gib), "--steps", str(steps),
-                        "--warmup", str(warmup)], stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900, env=env, cwd=ROOT)
+                        "--warmup", str(warmup), "--dump-outputs", str(tmp_path / "dump")], stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900, env=env, cwd=ROOT)
     assert p.returncode == 0, p.stderr[-3000:]
     lines = [l for l in p.stdout.splitlines() if l.strip()]
     assert len(lines) == 1, lines
@@ -67,16 +67,28 @@ def test_own_arm_control_flow_and_json_line_on_the_mock_runtime():
     assert d["gpu_launches"] > 0
     r = d["roofline"]
     assert r["bound"] == "hbm" and r["unit"] == "GB/s" and r["algorithmic_bytes_per_launch"] == n and r["launches_timed"] == 5
-    assert abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9 and "note" in r and r["traffic"] is None
+    assert abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9 and "note" in r
     assert d["resident_verify"]["value"] > 0
     for leg in ("e2e_reread", "e2e_pread", "e2e_framed"):
         assert d[leg]["unit"] == "GB/s" and d[leg]["value"] > 0 and d[leg]["steps"] == 2, leg
     assert set(d["clocks"]) >= {"sm_mhz", "sm_max_mhz", "reasons"}
     c = d["cpu_baseline"]
     assert c["kind"] == "port" and c["unit"] == "GB/s" and c["value"] > 0 and c["cores"] >= 2 and "pass" in c["sample"]
+    # --dump-outputs: the last headline step's buffer (sampled) and CRCs, float arrays, 64 MB at most
+    import numpy as np
+    files = {f.stem: np.load(f) for f in (tmp_path / "dump").iterdir()}
+    assert set(files) == {"dst_sample", "dst_sample_pos", "block_crc", "verify"} and sum(f.stat().st_size for f in (tmp_path / "dump").iterdir()) <= 64 << 20
+    assert all(a.dtype in (np.float32, np.float64) for a in files.values())
+    assert len(files["block_crc"]) == blocks and files["block_crc"].sum() == d["setup"]["sum_crc_last"] == files["verify"][0]
+    assert files["verify"].tolist() == [d["setup"]["sum_crc_last"], 0, blocks, n]
+    pos = files["dst_sample_pos"].astype(np.int64)
+    assert pos[0] == 0 and pos[-1] == n - 1 and np.all(np.diff(pos) >= 0)
+    from oracle import synth
+    want = np.frombuffer(synth.file_bytes(5000 + steps + warmup - 1, n, 4 << 20), dtype=np.uint8)
+    assert np.array_equal(files["dst_sample"], want[pos].astype(np.float32))
 
 
-def test_own_arm_two_ranks_on_the_mock_runtime():
+def test_own_arm_two_ranks_on_the_mock_runtime(tmp_path):
     """The N>1 launch the driver uses (torch.distributed.run, one rank per GPU) with world_size 2 on CPU: gloo stands in for NCCL, the
     mock runtime for the GPUs.  Rank 0 hosts the worker and generates the 2 x 0.25 GiB file, the manifest is broadcast, every rank
     reads its round-robin shard out of ITS arena dir, timings are max-reduced, rank 0 prints the one line."""
@@ -87,7 +99,8 @@ def test_own_arm_two_ranks_on_the_mock_runtime():
     port = s.getsockname()[1]
     s.close()
     p = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1", "--master-port", str(port),
-                        os.path.join(ROOT, "tests", "mock_cuda", "run_bench_on_mock.py"), "--gpus", "2", "--gib-per-gpu", "0.25", "--steps", "2", "--warmup", "1", "--side-steps", "1"],
+                        os.path.join(ROOT, "tests", "mock_cuda", "run_bench_on_mock.py"), "--gpus", "2", "--gib-per-gpu", "0.25", "--steps", "2", "--warmup", "1", "--side-steps", "1",
+                        "--dump-outputs", str(tmp_path / "dump")],
                        stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900, env=env, cwd=ROOT)
     assert p.returncode == 0, p.stderr[-3000:]
     lines = [l for l in p.stdout.splitlines() if l.strip().startswith("{")]
@@ -97,10 +110,21 @@ def test_own_arm_two_ranks_on_the_mock_runtime():
     assert d["n_gpus"] == 2 and d["scaling"] == "weak" and d["config"]["file_bytes"] == n and d["config"]["blocks_per_gpu"] == n // (4 << 20) // 2
     assert d["e2e"]["h2d_bytes_per_step"] == n and d["e2e"]["value"] > 0 and d["value"] > 0
     assert "cpu_baseline" not in d  # rank 0 at N=1 only
+    # every rank dumps its own shard; the sample is split between the ranks, so the whole dump stays within 64 MB
+    files = sorted(f.name for f in (tmp_path / "dump").iterdir())
+    assert files == sorted("%s_rank%d.npy" % (k, r) for k in ("dst_sample", "dst_sample_pos", "block_crc", "verify") for r in (0, 1))
+    assert sum(f.stat().st_size for f in (tmp_path / "dump").iterdir()) <= 64 << 20
+
+
+def test_dump_outputs_is_refused_where_it_has_nothing_to_write():
+    for extra in (["--impl", "reference"], ["--config", "c4"], ["--config", "c5"]):
+        p = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--dump-outputs", "/nonexistent/dump"] + extra,
+                           stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=120)
+        assert p.returncode == 2 and "--dump-outputs" in p.stderr and p.stdout == "", (extra, p.stderr[-500:])
 
 
 def test_smoke_control_flow_on_the_mock_runtime():
-    """__graft_entry__.smoke() end to end without a GPU (mock runtime): the three passes it makes on the B200 -- files tier short-circuit,
+    """__graft_entry__.smoke() end to end without a GPU (mock runtime): the three passes it makes on the H100 -- files tier short-circuit,
     files tier framed, arena tier DMA -- each land the oracle's bytes and CRC sums."""
     env = _shim_env()
     p = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "mock_cuda", "run_smoke_on_mock.py")], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,

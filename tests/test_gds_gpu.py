@@ -1,5 +1,5 @@
-"""SSD-tier blocks into HBM: GPUDirect Storage (cuFileRead, curvine_b200/csrc/host/gds.h) where the box offers it -- also in
-cuFile's compatibility mode with gds = "on" -- and the pinned ring otherwise.  Whatever path runs, bytes and CRCs must equal the
+"""SSD-tier blocks into HBM: GPUDirect Storage (cuFileRead, curvine_b200/csrc/host/gds.h) where the host offers it (nvidia-fs)
+and the pinned ring otherwise.  Whatever path runs, bytes and CRCs must equal the
 oracle's (SURVEY.md 8f-2; tier model: storage_info.rs:36-49, local_file.rs:202-213)."""
 import os
 import shutil
@@ -17,10 +17,6 @@ pytestmark = pytest.mark.gpu
 @pytest.mark.parametrize("gds", ["on", "off", "auto"])
 def test_ssd_tier_file_lands_bit_exact_whichever_path_serves_it(cuda, gds):
     import torch
-    if gds == "on" and not os.environ.get("CV_TEST_GDS_ON") and not os.environ.get("CV_TEST_MOCK_CUDA_LIB"):
-        # cuFile's compatibility mode could not be exercised on a B200 box before round 2 lost its GPU access (the one attempt was
-        # refused at cuFileHandleRegister and fell back to the ring, as designed): forcing it stays opt-in until it has been seen to work
-        pytest.skip("gds = on (cuFile compatibility mode) is opt-in: CV_TEST_GDS_ON=1")
     d = tempfile.mkdtemp(prefix="cvssd", dir=os.environ.get("CV_SSD_DIR", "/tmp"))  # a disk-backed directory, not tmpfs
     try:
         with F.MiniWorker(["[SSD]" + d]) as w:
@@ -41,7 +37,7 @@ def test_ssd_tier_file_lands_bit_exact_whichever_path_serves_it(cuda, gds):
                 assert got == n - 12345 and bad == 0 and ver == 6  # block 0 is partial
                 assert dst[:got].cpu().numpy().tobytes() == want[12345:]
                 st = r.device_stats()
-                may_gds = info["available"] and (gds == "on" or (gds == "auto" and not info["compat"]))
+                may_gds = info["available"] and gds != "off"
                 # either every byte went through cuFileRead, or cuFile turned the files away and every byte took the pinned ring
                 assert st["gds_bytes"] in ((0, got) if may_gds else (0,)), (st["gds_bytes"], F.gds_info(), gds)
                 r.complete()

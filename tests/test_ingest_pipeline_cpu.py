@@ -1,12 +1,12 @@
 """The GPU ingest pipeline's HOST logic on a machine without a GPU.
 
-tests/test_gpu_reader.py is the parity suite of the reader through the C ABI (`-m gpu`, run on a B200 against the real
+tests/test_gpu_reader.py is the parity suite of the reader through the C ABI (`-m gpu`, run on an H100 against the real
 library).  Here the same tests run in a subprocess against tests/mock_cuda's library: the product's C++ host side
 (csrc/host/*: job planning, pinned ring, copy groups, registrar, fetch threads, verify batching, result harvesting, the
 worker, the writer, the HBM tier) compiled against a host-memory stand-in for the CUDA runtime, with plain-loop CPU stand-ins
 for the cvk_* launchers instead of csrc/kernels.cu.  That checks the pipeline's bookkeeping (what lands where, which CRC is
 compared with which manifest entry, slot reuse, cache revalidation, error paths) on every CPU run; it says nothing about the
-kernels (tests/test_simt_emu.py runs the same suites against the kernel SOURCE on a SIMT shim; the B200 run checks the compiled code).  The mock is test infrastructure: nothing under curvine_b200/ can load it."""
+kernels (tests/test_simt_emu.py runs the same suites against the kernel SOURCE on a SIMT shim; the H100 run checks the compiled code).  The mock is test infrastructure: nothing under curvine_b200/ can load it."""
 import os
 import re
 import subprocess

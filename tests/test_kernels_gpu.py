@@ -1,4 +1,4 @@
-"""Parity of the sm_100a kernels (through the C ABI) against the CPU oracle.  Bit-exact: integer/byte work."""
+"""Parity of the sm_90a kernels (through the C ABI) against the CPU oracle.  Bit-exact: integer/byte work."""
 import zlib
 
 import numpy as np

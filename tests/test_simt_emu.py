@@ -1,6 +1,6 @@
 """The product's KERNEL SOURCE on a machine without a GPU.
 
-tests/simt_emu compiles curvine_b200/csrc/kernels.cu -- the file nvcc compiles for sm_100a, unmodified apart from a mechanical
+tests/simt_emu compiles curvine_b200/csrc/kernels.cu -- the file nvcc compiles for sm_90a, unmodified apart from a mechanical
 rewrite of the launch syntax and of the inline PTX -- for host cores on a SIMT shim: a fiber per CUDA thread, blocks spread over
 host threads, __syncthreads / __syncwarp / *_sync warp intrinsics completing exactly when every live participant has arrived.
 The whole `-m gpu` suite (kernel parity against the oracle, the reader through the C ABI, arena, GDS fallback, faults, the
@@ -8,7 +8,7 @@ two-device gather) then runs in a subprocess against that library -- with the ru
 (tests/mock_cuda/mock_cuda.cc: a thread per stream, random pauses, ordering only through events), so the pipeline's stream
 dependencies are exercised too.  This checks the kernels' ALGORITHM (index math, shuffle
 patterns, the GF(2) folds, barrier placement) on every CPU run; what it cannot check is what only the hardware decides (memory
-model races between unsynchronised threads, the compiled SASS, speed) -- the B200 run of the same tests covers that.
+model races between unsynchronised threads, the compiled SASS, speed) -- the H100 run of the same tests covers that.
 Test infrastructure: nothing under curvine_b200/ can load this library."""
 import os
 import re

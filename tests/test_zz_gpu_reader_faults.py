@@ -1,5 +1,5 @@
 """Fault injection and cache-policy checks of the GPU reader through the C ABI (dead workers, fail-over, recovery, registration cache
-admission).  Collected last (zz) so the established parity suites run first; runs on a B200 (`-m gpu`) and, through
+admission).  Collected last (zz) so the established parity suites run first; runs on an H100 (`-m gpu`) and, through
 tests/test_ingest_pipeline_cpu.py, against the mock runtime on CPU."""
 import os
 import threading

@@ -145,8 +145,9 @@ def test_plain_c_host_example_reads_a_file_into_device_memory(cuda):
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     lib = os.environ.get("CV_TEST_MOCK_CUDA_LIB") or os.path.join(root, "curvine_b200", "libcurvine_b200.so")
     d = tempfile.mkdtemp(prefix="cvch", dir="/dev/shm" if os.path.isdir("/dev/shm") else None)
+    bin_dir = tempfile.mkdtemp(prefix="cvch_bin")  # not under /dev/shm, which may be mounted noexec
     try:
-        exe = os.path.join(d, "c_host")
+        exe = os.path.join(bin_dir, "c_host")
         cc = subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-pedantic", "-Werror", "-I", os.path.join(root, "include"), os.path.join(root, "examples", "c_host.c"),
                              "-o", exe, "-L", os.path.dirname(lib), "-l:" + os.path.basename(lib), "-Wl,-rpath," + os.path.dirname(lib)],
                             stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
@@ -173,3 +174,4 @@ def test_plain_c_host_example_reads_a_file_into_device_memory(cuda):
             assert r.returncode == 1 and "cv_open" in r.stdout and "-8" in r.stdout, r.stdout   # FileNotFound, reported through cv_last_error
     finally:
         shutil.rmtree(d, ignore_errors=True)
+        shutil.rmtree(bin_dir, ignore_errors=True)

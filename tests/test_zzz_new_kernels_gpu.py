@@ -1,6 +1,6 @@
-"""Round-2 kernels that no B200 run has checked in isolation yet (round 2 lost its GPU access after they were written; the product paths
-that use them -- small-file reads, FUSE page scatter, the 262,144-page kbench case -- did run green on the GPU).  The file sorts after the
-established suites on purpose: whatever happens here, everything else has already run.
+"""The newer kernels checked in isolation (the product paths that use them -- small-file reads, FUSE page scatter, the 262,144-page
+kbench case -- are covered by the reader suites too).  The file sorts after the established suites on purpose: whatever happens here,
+everything else has already run.
 
   * crc_small_kernel / gather_small_kernel: the single-launch small-input kernels, against the oracle and against the launch train
   * the multi-CTA prefix scan (more than 16 Ki pieces)"""

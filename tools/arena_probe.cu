@@ -91,14 +91,7 @@ int main(int argc, char** argv) {
             if (l.find("Huge") != std::string::npos || l.find("Shmem") != std::string::npos) printf("    %s\n", l.c_str());
     }
     {
-        int fd = open("/proc/sys/vm/nr_hugepages", O_WRONLY);
-        if (fd < 0) printf("A nr_hugepages not writable: %s\n", strerror(errno));
-        else {
-            ssize_t w = write(fd, "2048\n", 5);
-            printf("A wrote nr_hugepages=2048 -> %zd (%s)\n", w, w < 0 ? strerror(errno) : "ok");
-            close(fd);
-            cat("/proc/sys/vm/nr_hugepages");
-        }
+        // uses whatever hugetlb pool the host already has; the probe never changes host settings
         int mfd = memfd_create("hp", MFD_HUGETLB);
         if (mfd < 0) printf("A memfd_create(MFD_HUGETLB): %s\n", strerror(errno));
         else {

@@ -7,7 +7,7 @@ and the same two cases for the reference-shaped CPU reader (oracle/cpu_reader.c)
   gds    [b200] gds = on|off|auto: cuFileRead straight into HBM (curvine_b200/csrc/host/gds.h) vs the pinned ring
   hbm    (--hbm) the worker's HBM tier over the SSD tier: framed reads cold from the disk, then -- after asynchronous promotion
          (hbm_promote_after = 1) -- served out of HBM as K4-packed frames; hit rate and GB/s per pass.
-BASELINE.json names 128 GiB over 8 GPUs; the GPU box has a 79 GB overlay disk, so the size is a parameter (default 16 GiB)."""
+BASELINE.json names 128 GiB over 8 GPUs; a host's disk may not hold that, so the size is a parameter (default 16 GiB)."""
 import argparse
 import glob
 import json

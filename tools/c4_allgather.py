@@ -1,6 +1,9 @@
 """Config C4 (model distribution): a checkpoint file, mem tier, every GPU ends up holding ALL bytes in file order.
 
-  torchrun --nproc-per-node G tools/c4_allgather.py --gib 70
+  torchrun --nproc-per-node G tools/c4_allgather.py --gib 32
+
+Every GPU holds the whole file twice over (the file-order result and the all-gather staging buffer) plus its shard, so 32 GiB
+is the largest power of two that fits an 80 GB H100.
 
 Each rank ingests its round-robin shard (cv_read_device_sharded, CRC-32C verified on the GPU), then the exchange runs two ways:
   A  NCCL all_gather_into_tensor (in place) + cvk_deinterleave_blocks            (collective, then a 2N HBM pass)
@@ -22,13 +25,13 @@ BLOCK = 4 << 20
 
 def main_bench(args, emit):
     """bench.py --config c4: the same measurement, printed as ONE line in the bench contract (rank 0)."""
-    a = argparse.Namespace(gib=70.0 if args.gib_per_gpu == 16.0 else args.gib_per_gpu * args.gpus, skip_nccl=False, arena=args.tier == "arena", emit=emit)
+    a = argparse.Namespace(gib=32.0 if args.gib_per_gpu == 16.0 else args.gib_per_gpu * args.gpus, skip_nccl=False, arena=args.tier == "arena", emit=emit)
     return run(a)
 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--gib", type=float, default=70.0)
+    ap.add_argument("--gib", type=float, default=32.0)
     ap.add_argument("--skip-nccl", action="store_true")
     ap.add_argument("--arena", type=int, default=1, help="mem tier = pinned-once arenas (one per GPU) instead of one tmpfs file per block")
     a = ap.parse_args()
@@ -187,7 +190,7 @@ def run(a):
                                    % (n / 2 ** 30, "arena" if a.arena else "files"), "file_bytes": n, "block_bytes": BLOCK},
             "ingest": {"first_read_ms": res["ingest_ms_rep0"], "first_read_GBps": n / res["ingest_ms_rep0"] / 1e6, "reread_ms": res["ingest_ms_rep1"], "mount_ms": res.get("mount_ms")},
             "exchange_p2p_fused": {"ms": res["p2p_gather_ms_rep2"], "GBps_into_each_gpu": res["p2p_gather_GBps_into_each_gpu"],
-                                   "nvlink_GBps_per_gpu": res["p2p_nvlink_GBps_per_gpu"], "frac_of_nvlink5_900GBps": res["p2p_nvlink_GBps_per_gpu"] / 900.0,
+                                   "nvlink_GBps_per_gpu": res["p2p_nvlink_GBps_per_gpu"], "frac_of_nvlink4_450GBps": res["p2p_nvlink_GBps_per_gpu"] / 450.0,
                                    "what": "cvk_gather_shards_p2p: one K3-bodied kernel per GPU reads every block out of its owner's HBM (peer pointers, symmetric memory) into file order"},
             "exchange_nccl": {"allgather_ms": res.get("nccl_allgather_ms_rep1"), "deinterleave_ms": res.get("deinterleave_ms_rep1"), "total_ms": res.get("nccl_total_ms"),
                               "what": "all_gather_into_tensor + cvk_deinterleave_blocks"},

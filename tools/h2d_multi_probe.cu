@@ -3,7 +3,7 @@
 // of GPUs behind one PCIe switch less than 2 x the solo rate" from "our pipeline loses something when it is not alone".
 //   per GPU: one thread bound to the GPU's NUMA node, 4 pinned buffers of 32 MiB allocated from that thread, one stream,
 //   cudaMemcpyAsync round-robin for ~1.5 s, CUDA events for the device-side time.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/h2d_multi_probe tools/h2d_multi_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/h2d_multi_probe tools/h2d_multi_probe.cu
 // Run:   tools/h2d_multi_probe            (sweeps the first 1, 2, 4, 8 devices and prints per-GPU GB/s)
 #include <cuda_runtime.h>
 #include <sched.h>

@@ -1,9 +1,9 @@
-// Access-pattern probe: how much HBM copy bandwidth does a persistent 148 x 1024-thread kernel get on B200 when
+// Access-pattern probe: how much HBM copy bandwidth does a persistent one-CTA-per-SM x 1024-thread kernel get when
 //   A  the whole grid streams through memory together (grid-stride, 4 rows per thread in flight)
 //   B  every WARP walks a private contiguous region (4736 concurrent read streams + 4736 write streams), tiles of 4 rows
-//   C  every CTA walks a private contiguous region, its 32 warps taking adjacent 512-byte rows (148 streams)
+//   C  every CTA walks a private contiguous region, its 32 warps taking adjacent 512-byte rows (one stream per SM)
 //   D  like B with 64 KiB segments handed out round-robin inside a CTA's range (the layout of walk_kernel)
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/pattern_probe tools/pattern_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/pattern_probe tools/pattern_probe.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>

@@ -6,11 +6,11 @@ ROOT="$(cd "$(dirname "$0")/.." && pwd)"
 W=/tmp/cv_asan; mkdir -p $W; cd $W
 for f in $ROOT/curvine_b200/csrc/kernels.cu $ROOT/curvine_b200/csrc/host/*.cu $ROOT/curvine_b200/csrc/host/*.cc; do
   x=cu; case $f in *.cc) x=c++;; esac
-  nvcc -gencode arch=compute_100a,code=sm_100a -O1 -g -std=c++17 \
+  nvcc -gencode arch=compute_90a,code=sm_90a -O1 -g -std=c++17 \
     -Xcompiler -fPIC,-pthread,-msse4.2,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer -cudart static \
     -I $ROOT/include -I $ROOT/curvine_b200/csrc -x $x -c $f -o $(basename $f).o &
 done; wait
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -cudart static -Xcompiler -fsanitize=address,-fsanitize=undefined -o asan.so *.o -lpthread -ldl -lrt
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -cudart static -Xcompiler -fsanitize=address,-fsanitize=undefined -o asan.so *.o -lpthread -ldl -lrt
 cp $ROOT/curvine_b200/libcurvine_b200.so orig.so; cp asan.so $ROOT/curvine_b200/libcurvine_b200.so
 trap "cp $W/orig.so $ROOT/curvine_b200/libcurvine_b200.so" EXIT
 cd $ROOT
