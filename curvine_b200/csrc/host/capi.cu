@@ -337,6 +337,56 @@ int64_t cv_shard_plan(cv_reader* r, int32_t rank, int32_t world, int64_t* block_
     API_GUARD_END
 }
 
+static std::vector<ReadvRange> readv_ranges(const CvRange* ranges, int32_t n) {
+    std::vector<ReadvRange> out;
+    for (int32_t i = 0; ranges && i < n; i++) out.push_back(ReadvRange{ranges[i].file_off, ranges[i].len, static_cast<uint8_t*>(ranges[i].d_dst)});
+    return out;
+}
+
+int64_t cv_readv_device(cv_reader* r, const CvRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes) {
+    API_GUARD_BEGIN
+    API_NEED(r);
+    API_NEED(nbytes);
+    if (n > 0) API_NEED(ranges);
+    API_TRY(ensure_dev(r));
+    const std::vector<ReadvRange> rs = readv_ranges(ranges, n);
+    int64_t got = 0;
+    API_TRY(r->dev->readv_device(rs.data(), n, stream, &got));
+    *nbytes = got;
+    return ok();
+    API_GUARD_END
+}
+
+int64_t cv_readv_plan(cv_reader* r, const CvRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len, int32_t* range_index,
+                      int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes) {
+    API_GUARD_BEGIN
+    API_NEED(r);
+    if (n > 0) API_NEED(ranges);
+    const std::vector<ReadvRange> rs = readv_ranges(ranges, n);
+    const FileBlocks& fb = r->host->file_blocks();
+    std::vector<ReadvBlock> blocks;
+    std::vector<ReadvSpan> spans;
+    API_TRY(plan_readv(fb, rs.data(), n, &blocks, &spans));
+    int64_t fetched = 0;
+    size_t i = 0;
+    for (const ReadvBlock& b : blocks) {
+        fetched += fb.block_locs[b.block].block.len;
+        for (size_t k = b.first_span; k < b.first_span + b.n_spans; k++, i++) {
+            if (i >= static_cast<size_t>(std::max(cap, 0))) continue;
+            if (block_index) block_index[i] = static_cast<int64_t>(b.block);
+            if (block_off) block_off[i] = spans[k].block_off;
+            if (len) len[i] = spans[k].len;
+            if (range_index) range_index[i] = spans[k].range;
+            if (direct) direct[i] = b.direct ? 1 : 0;
+        }
+    }
+    if (n_spans) *n_spans = static_cast<int32_t>(spans.size());
+    if (n_blocks) *n_blocks = static_cast<int64_t>(blocks.size());
+    if (fetch_bytes) *fetch_bytes = fetched;
+    return ok();
+    API_GUARD_END
+}
+
 int64_t cv_fuse_read_device(cv_reader* r, int64_t pos, int64_t len, void* d_scratch, void* d_page_base, const uint64_t* page_offsets,
                             int32_t n_pages, int64_t page_size, cv_stream_t stream, int64_t* nbytes) {
     API_GUARD_BEGIN

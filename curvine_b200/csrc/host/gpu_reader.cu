@@ -8,6 +8,7 @@
 #include <sys/stat.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <deque>
 #include <list>
 #include <set>
@@ -505,6 +506,20 @@ class GpuIngest {
     bool register_inline = false;
     std::atomic<int> reads_in_flight{0};  // run_jobs calls between entry and return (the registrar yields to them)
     double ring_alloc_sec = 0;            // time spent allocating the pinned ring (one-off per context and slot size)
+    // device staging of the boundary blocks of vectored reads (readv_device): one vectored read at a time uses it, under readv_mu
+    std::mutex readv_mu;
+    uint8_t* d_readv_stage = nullptr;
+    size_t d_readv_stage_bytes = 0;
+
+    Err ensure_readv_stage(size_t bytes) {
+        if (bytes <= d_readv_stage_bytes) return Err::ok();
+        CU_TRY(cudaDeviceSynchronize());  // an earlier vectored read's K3 may still be reading the old staging
+        if (d_readv_stage) cudaFree(d_readv_stage);
+        d_readv_stage = nullptr, d_readv_stage_bytes = 0;
+        CU_TRY(cudaMalloc(&d_readv_stage, bytes));
+        d_readv_stage_bytes = bytes;
+        return Err::ok();
+    }
 
     Err ensure_tables(size_t tables_bytes, size_t result_bytes) {
         if (tables_bytes > d_tables_cap) {
@@ -623,6 +638,7 @@ class GpuIngest {
         reg.clear();
         if (pinned) cudaFreeHost(pinned);
         if (d_stage) cudaFree(d_stage);
+        if (d_readv_stage) cudaFree(d_readv_stage);
         if (d_tables) cudaFree(d_tables);
         if (h_result) cudaFreeHost(h_result);
         if (h_tables) cudaFreeHost(h_tables);
@@ -734,14 +750,16 @@ Err GpuFsReader::fuse_read_device(int64_t want, void* d_scratch, void* d_page_ba
     const int64_t take = std::max<int64_t>(0, std::min(want, len() - pos_));
     const int64_t need_pages = (take + page_size - 1) / page_size;
     if (need_pages > n_pages) return Err::common("not enough page buffers for the reply");
-    PageScatter ps;
-    ps.d_page_base = static_cast<uint8_t*>(d_page_base), ps.page_offsets = page_offsets, ps.n_pages = need_pages, ps.page_size = page_size, ps.total = take;
+    Scatter ps;
+    ps.d_out = static_cast<uint8_t*>(d_page_base), ps.total = static_cast<uint64_t>(take);
+    for (int64_t i = 0; i < need_pages; i++)
+        ps.segs.push_back(CvSeg{static_cast<uint64_t>(i * page_size), page_offsets[i], static_cast<uint64_t>(std::min(page_size, take - i * page_size))});
     return read_device_impl(d_scratch, take, stream, n, need_pages > 0 ? &ps : nullptr);
 }
 
 Err GpuFsReader::read_device(void* d_dst, int64_t cap, void* stream, int64_t* n) { return read_device_impl(d_dst, cap, stream, n, nullptr); }
 
-Err GpuFsReader::read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const PageScatter* pages) {
+Err GpuFsReader::read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const Scatter* pages) {
     *n = 0;
     const int64_t end = std::min(len(), pos_ + std::max<int64_t>(cap, 0));
     if (end <= pos_) return Err::ok();
@@ -785,6 +803,42 @@ Err GpuFsReader::read_device_sharded(int rank, int world, void* d_dst, int64_t c
     for (const auto& p : plan) jobs.push_back(Job{&(*fbp_).block_locs[p.block], 0, p.len, p.dst_off, true});
     CV_RETURN_IF_ERR(run_jobs(jobs, static_cast<uint8_t*>(d_dst), stream));
     *n = total;
+    return Err::ok();
+}
+
+Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::vector<ReadvBlock>* blocks, std::vector<ReadvSpan>* spans) {
+    blocks->clear(), spans->clear();
+    if (n < 0) return Err::common(str_printf("readv: negative range count %d", n));
+    if (n > 0 && !ranges) return Err::common("readv: null range table");
+    const int64_t flen = fb.status.len;
+    std::vector<int32_t> order;
+    for (int32_t i = 0; i < n; i++) {
+        const ReadvRange& r = ranges[i];
+        if (r.len < 0) return Err::common(str_printf("readv: range %d has a negative length (%lld)", i, (long long)r.len));
+        if (r.file_off < 0 || r.file_off > flen || r.len > flen - r.file_off)
+            return Err::common(str_printf("readv: range %d [%lld, +%lld) lies outside the file (%lld bytes)", i, (long long)r.file_off, (long long)r.len, (long long)flen));
+        if (r.len > 0) order.push_back(i);
+    }
+    std::sort(order.begin(), order.end(), [&](int32_t a, int32_t b) { return ranges[a].file_off < ranges[b].file_off; });
+    for (size_t k = 1; k < order.size(); k++)
+        if (ranges[order[k]].file_off < ranges[order[k - 1]].file_off + ranges[order[k - 1]].len)
+            return Err::common(str_printf("readv: ranges %d and %d overlap in the file", order[k - 1], order[k]));
+    for (int32_t i : order) {
+        for (int64_t p = ranges[i].file_off, end = p + ranges[i].len; p < end;) {
+            int64_t boff;
+            size_t idx;
+            CV_RETURN_IF_ERR(fb.get_read_block(p, &boff, &idx));
+            const int64_t take = std::min(end - p, fb.block_locs[idx].block.len - boff);
+            if (blocks->empty() || blocks->back().block != idx) blocks->push_back(ReadvBlock{idx, false, spans->size(), 0});
+            spans->push_back(ReadvSpan{boff, take, i});
+            blocks->back().n_spans++;
+            p += take;
+        }
+    }
+    for (ReadvBlock& b : *blocks) {
+        const ReadvSpan& s = (*spans)[b.first_span];
+        b.direct = b.n_spans == 1 && s.block_off == 0 && s.len == fb.block_locs[b.block].block.len;
+    }
     return Err::ok();
 }
 
@@ -954,7 +1008,18 @@ Err GpuFsReader::verify(uint64_t* sum_crc, uint32_t* n_bad, uint64_t* n_verified
     return e;
 }
 
-Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* user_stream, const PageScatter* pages) {
+// `p` must be device memory on `device`
+static Err check_device_dst(const void* p, int device) {
+    cudaPointerAttributes pa;
+    if (cudaPointerGetAttributes(&pa, p) != cudaSuccess || pa.type != cudaMemoryTypeDevice) {
+        cudaGetLastError();
+        return Err::common("cv_read_device: destination is not device memory");
+    }
+    if (pa.device != device) return Err::common(str_printf("cv_read_device: destination lives on device %d but [b200] device = %d", pa.device, device));
+    return Err::ok();
+}
+
+Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* user_stream, const Scatter* pages) {
     const size_t J = jobs.size();
     if (J == 0) return Err::ok();
     const double t_start = now_sec();
@@ -966,15 +1031,7 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     } in_flight(G.reads_in_flight);
     std::lock_guard<std::mutex> call_lock(G.mu);
     CU_TRY(cudaSetDevice(G.device));
-    {
-        cudaPointerAttributes pa;
-        if (cudaPointerGetAttributes(&pa, d_dst) != cudaSuccess || pa.type != cudaMemoryTypeDevice) {
-            cudaGetLastError();
-            return Err::common("cv_read_device: destination is not device memory");
-        }
-        if (pa.device != G.device)
-            return Err::common(str_printf("cv_read_device: destination lives on device %d but [b200] device = %d", pa.device, G.device));
-    }
+    CV_RETURN_IF_ERR(check_device_dst(d_dst, G.device));
     if (G.pending_owner && G.pending_owner != this) CV_RETURN_IF_ERR(G.pending_owner->harvest());  // shared tables
     CV_RETURN_IF_ERR(harvest());
     // everything this call writes into d_dst is ordered after what the caller's stream had queued at entry (a buffer fresh from
@@ -1045,7 +1102,7 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     const size_t o_off = 0, o_len = up(o_off + 8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_crc = up(o_skip + J);
     const size_t res_words = J + 4 + F;
     const size_t o_streams = up(o_crc + 4 * res_words), o_fdesc = up(o_streams + sizeof(CvStreamDesc) * J);
-    const size_t n_segs = pages ? static_cast<size_t>(pages->n_pages) : 0;
+    const size_t n_segs = pages ? pages->segs.size() : 0;
     const size_t o_segs = up(o_fdesc + sizeof(CvFrameDesc) * F);
     const size_t tables_bytes = up(o_segs + sizeof(CvSeg) * n_segs);
     CV_RETURN_IF_ERR(G.ensure_tables(tables_bytes, 4 * res_words));
@@ -1074,12 +1131,9 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     // masked out one by one (their CRCs are still computed, and summed when they lie inside [f0,f1))
     const bool compare = bc.verify && n_compared > 0;
     CU_TRY(cudaMemcpyAsync(T, h, o_crc, cudaMemcpyHostToDevice, G.vstream));
-    if (n_segs) {  // the page scatter's segment table rides in the same pinned image
+    if (n_segs) {  // the scatter's segment table rides in the same pinned image
         CvSeg* hs = reinterpret_cast<CvSeg*>(h + o_segs);
-        for (size_t i = 0; i < n_segs; i++) {
-            hs[i].src_off = static_cast<uint64_t>(i) * static_cast<uint64_t>(pages->page_size), hs[i].dst_off = pages->page_offsets[i];
-            hs[i].len = static_cast<uint64_t>(std::min<int64_t>(pages->page_size, pages->total - static_cast<int64_t>(i) * pages->page_size));
-        }
+        memcpy(hs, pages->segs.data(), sizeof(CvSeg) * n_segs);
         CU_TRY(cudaMemcpyAsync(T + o_segs, hs, sizeof(CvSeg) * n_segs, cudaMemcpyHostToDevice, G.vstream));
     }
     CU_TRY(cudaMemsetAsync(T + o_crc, 0, 4 * res_words, G.vstream));
@@ -1461,9 +1515,8 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     if (compare)
         CVK_TRY(cvk_verify_crcs_masked(d_crc + f0, reinterpret_cast<const uint32_t*>(T + o_exp) + f0, T + o_skip + f0, static_cast<uint32_t>(f1 - f0), d_crc + J, nullptr,
                                        G.vstream));
-    if (n_segs)  // every copy group was waited for and CRC'd on vstream by now: scatter the landed bytes into the page buffers
-        CVK_TRY(cvk_gather_pages(d_dst, reinterpret_cast<const CvSeg*>(T + o_segs), static_cast<uint32_t>(n_segs), static_cast<uint64_t>(pages->total), pages->d_page_base,
-                                 G.vstream));
+    if (n_segs)  // every copy group was waited for and CRC'd on vstream by now: scatter the landed bytes to their destinations
+        CVK_TRY(cvk_gather_pages(d_dst, reinterpret_cast<const CvSeg*>(T + o_segs), static_cast<uint32_t>(n_segs), pages->total, pages->d_out, G.vstream));
     CU_TRY(cudaMemcpyAsync(G.h_result, d_crc, 4 * res_words, cudaMemcpyDeviceToHost, G.vstream));
     CU_TRY(cudaEventRecord(G.done_ev, G.vstream));
     CU_TRY(cudaStreamWaitEvent(static_cast<cudaStream_t>(user_stream), G.done_ev, 0));
@@ -1506,6 +1559,69 @@ Err GpuFsReader::read_many(FsContext* ctx, const std::vector<std::string>& paths
     CV_RETURN_IF_ERR(r->run_jobs(jobs, static_cast<uint8_t*>(d_dst), stream));
     if (total_bytes) *total_bytes = total;
     return r->verify(sum_crc, n_bad, n_verified);
+}
+
+// Upper bound of the boundary-block staging of a vectored read, besides "no more blocks than the pinned ring has slots".
+static const int64_t kReadvStageBytes = 256 << 20;
+
+Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* stream, int64_t* n) {
+    *n = 0;
+    const FileBlocks& fb = *fbp_;
+    std::vector<ReadvBlock> blocks;
+    std::vector<ReadvSpan> spans;
+    CV_RETURN_IF_ERR(plan_readv(fb, ranges, n_ranges, &blocks, &spans));
+    GpuIngest& G = *ing_;
+    CU_TRY(cudaSetDevice(G.device));
+    int64_t total = 0;
+    uintptr_t lo = UINTPTR_MAX;
+    for (int32_t i = 0; i < n_ranges; i++) {
+        if (ranges[i].len == 0) continue;
+        CV_RETURN_IF_ERR(check_device_dst(ranges[i].dst, G.device).ctx(str_printf("range %d", i)));
+        CV_RETURN_IF_ERR(check_device_dst(ranges[i].dst + ranges[i].len - 1, G.device).ctx(str_printf("range %d (last byte)", i)));
+        lo = std::min(lo, reinterpret_cast<uintptr_t>(ranges[i].dst));
+        total += ranges[i].len;
+    }
+    if (blocks.empty()) return Err::ok();
+    std::vector<size_t> boundary;
+    int64_t stage_block = 0;
+    for (size_t b = 0; b < blocks.size(); b++)
+        if (!blocks[b].direct) boundary.push_back(b), stage_block = std::max(stage_block, fb.block_locs[blocks[b].block].block.len);
+    // One run_jobs call per round: the direct blocks and the first round of boundary blocks go in the first; later rounds reuse the
+    // staging once the previous round's K3 has delivered it (run_jobs harvests the previous call on entry).
+    std::lock_guard<std::mutex> lk(G.readv_mu);
+    size_t per_round = 0;
+    uint8_t* stage = nullptr;
+    if (!boundary.empty()) {
+        per_round = std::min(boundary.size(), static_cast<size_t>(std::max<int64_t>(1, std::min<int64_t>(G.nslots, kReadvStageBytes / stage_block))));
+        CV_RETURN_IF_ERR(G.ensure_readv_stage(per_round * static_cast<size_t>(stage_block)));
+        stage = G.d_readv_stage;
+        lo = std::min(lo, reinterpret_cast<uintptr_t>(stage));
+    }
+    // every destination is addressed relative to the lowest one (or the staging): one base pointer, unsigned offsets
+    uint8_t* base = reinterpret_cast<uint8_t*>(lo);
+    auto rel = [lo](const uint8_t* p) { return static_cast<int64_t>(reinterpret_cast<uintptr_t>(p) - lo); };
+    auto dst_of = [&](const ReadvBlock& b, const ReadvSpan& s) { return rel(ranges[s.range].dst) + fb.starts[b.block] + s.block_off - ranges[s.range].file_off; };
+    std::vector<Job> jobs;
+    for (const ReadvBlock& b : blocks)
+        if (b.direct) jobs.push_back(Job{&fb.block_locs[b.block], 0, spans[b.first_span].len, dst_of(b, spans[b.first_span]), true});
+    size_t next = 0;
+    do {
+        Scatter sc;
+        sc.d_out = base;
+        for (size_t slot = 0; slot < per_round && next < boundary.size(); slot++, next++) {
+            const ReadvBlock& b = blocks[boundary[next]];
+            const int64_t at = rel(stage + slot * static_cast<size_t>(stage_block));
+            jobs.push_back(Job{&fb.block_locs[b.block], 0, fb.block_locs[b.block].block.len, at, true});
+            for (size_t k = b.first_span; k < b.first_span + b.n_spans; k++) {
+                sc.segs.push_back(CvSeg{static_cast<uint64_t>(at + spans[k].block_off), static_cast<uint64_t>(dst_of(b, spans[k])), static_cast<uint64_t>(spans[k].len)});
+                sc.total += static_cast<uint64_t>(spans[k].len);
+            }
+        }
+        CV_RETURN_IF_ERR(run_jobs(jobs, base, stream, sc.segs.empty() ? nullptr : &sc));
+        jobs.clear();
+    } while (next < boundary.size());
+    *n = total;
+    return Err::ok();
 }
 
 }  // namespace cv

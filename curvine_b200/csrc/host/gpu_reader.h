@@ -16,6 +16,7 @@
 #include <condition_variable>
 #include <thread>
 
+#include "../../../include/curvine_b200_kernels.h"
 #include "client.h"
 
 namespace cv {
@@ -45,6 +46,26 @@ struct ShardJob {
 };
 Err plan_shard(const FileBlocks& fb, int rank, int world, int64_t cap, std::vector<ShardJob>* out, int64_t* total);
 
+// Vectored read: n byte ranges of one file -> n destinations.  The plan lists every block a range touches, in file order, with the
+// spans of it that go to which range.  A block is direct when one range covers all of it: it lands in place as an ordinary whole-block
+// job.  Every other touched block is a boundary block: it is fetched whole into device staging, verified there like any whole block,
+// and its spans are delivered from the staging by K3.
+struct ReadvRange {
+    int64_t file_off, len;
+    uint8_t* dst;
+};
+struct ReadvSpan {
+    int64_t block_off, len;  // bytes [block_off, block_off + len) of the block
+    int32_t range;           // go to ranges[range].dst + (block start + block_off - ranges[range].file_off)
+};
+struct ReadvBlock {
+    size_t block;  // index into FileBlocks::block_locs
+    bool direct;
+    size_t first_span, n_spans;
+};
+// Ranges may come in any order; a negative length, a range outside the file or two ranges that overlap in the file is an error.
+Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::vector<ReadvBlock>* blocks, std::vector<ReadvSpan>* spans);
+
 class GpuIngest;  // per-FsContext pinned ring + streams
 struct RegMapping;
 
@@ -65,6 +86,9 @@ class GpuFsReader {
     // Round-robin shard of the whole file: blocks b with b % world == rank land back to back in slots of
     // block_size bytes (slot j = block j*world + rank).  *n = bytes landed (sum of those block lengths).
     Err read_device_sharded(int rank, int world, void* d_dst, int64_t cap, void* stream, int64_t* n);
+    // Vectored read (plan_readv): every touched block is fetched once and its CRC compared over the whole block.  Ordered on `stream`
+    // when the call returns; does not move pos.  *n = sum of the range lengths.
+    Err readv_device(const ReadvRange* ranges, int32_t n_ranges, void* stream, int64_t* n);
     // Waits for outstanding work; sum_crc = u64 sum of the per-block CRCs computed so far (verify_poly),
     // n_bad = blocks whose CRC differed from the manifest.
     Err verify(uint64_t* sum_crc, uint32_t* n_bad, uint64_t* n_verified);
@@ -84,15 +108,16 @@ class GpuFsReader {
         bool full;           // whole block -> CRC comparable with the manifest
     };
     GpuFsReader() = default;
-    // page scatter riding on a read (Reader::fuse_read + ResponseData::as_iovec on the device): after the bytes landed in d_dst
-    // and were CRC'd, segment i of d_dst goes to d_page_base + page_offsets[i] (K3), in the same launch train, no extra sync
-    struct PageScatter {
-        uint8_t* d_page_base = nullptr;
-        const uint64_t* page_offsets = nullptr;
-        int64_t n_pages = 0, page_size = 0, total = 0;
+    // scatter riding on a read: after the bytes landed in d_dst and were CRC'd, segs[i] copies d_dst + src_off to d_out + dst_off
+    // (K3), in the same launch train, no extra sync.  Page buffers of a FUSE reply (Reader::fuse_read + ResponseData::as_iovec on the
+    // device), or the spans of the boundary blocks of a vectored read.
+    struct Scatter {
+        uint8_t* d_out = nullptr;
+        std::vector<CvSeg> segs;
+        uint64_t total = 0;  // sum of segs[i].len
     };
-    Err run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* stream, const PageScatter* pages = nullptr);
-    Err read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const PageScatter* pages);
+    Err run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* stream, const Scatter* scatter = nullptr);
+    Err read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const Scatter* scatter);
     FsContext* ctx_ = nullptr;
     std::shared_ptr<const FileBlocks> fbp_;
     int64_t pos_ = 0;

@@ -8,7 +8,8 @@ Two deliberate differences, both stated where they occur:
     (curvinefs/curvineReader.py:49), which silently corrupts binary data; it also hands out `length` bytes from the address of ONE
     native chunk whatever its size (curvineReader.py:25-36).  Here `read(offset, length)` means what its arguments say: skip `offset`
     bytes from the current position, return up to `length` bytes, stop at end of file.
-  * read_tensor / read_range_tensor (additions): the bytes as a uint8 CUDA tensor in HBM, CRC-verified on the GPU, DLPack-exportable."""
+  * read_tensor / read_range_tensor (additions): the bytes as a uint8 CUDA tensor in HBM, CRC-verified on the GPU, DLPack-exportable.
+  * load_safetensors (addition): a safetensors checkpoint as {name: CUDA tensor} from one CRC-verified vectored read."""
 from typing import Optional
 
 from . import fs as _fs
@@ -164,6 +165,14 @@ class CurvineClient:
             return reader.read_tensor(length, device)
         finally:
             reader.close()
+
+    def load_safetensors(self, path, device=None, names=None):
+        """Addition: a safetensors checkpoint as {name: CUDA tensor}, from one CRC-verified vectored read (curvine_b200.safetensors)."""
+        from . import safetensors
+        try:
+            return safetensors.load_file(self.file_system_ptr, path, device=device, names=names)
+        except _fs.FsError as e:
+            raise IOError("Native load safetensors failed: %s" % e)
 
     def close(self):
         if self.file_system_ptr is not None:

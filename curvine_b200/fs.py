@@ -174,6 +174,35 @@ class Reader:
         _check(_lib.lib().cv_shard_plan(self._h, rank, world, arrs[0], arrs[1], arrs[2], arrs[3], n.value, ctypes.byref(n), ctypes.byref(tot)))
         return [tuple(a[i] for a in arrs) for i in range(n.value)]
 
+    @staticmethod
+    def _ranges(ranges):
+        arr = (_lib.CvRange * max(1, len(ranges)))()
+        for i, (off, n, ptr) in enumerate(ranges):
+            arr[i].file_off, arr[i].len, arr[i].d_dst = off, n, ptr
+        return arr
+
+    def readv_device(self, ranges, stream: int = 0) -> int:
+        """Vectored device read: `ranges` is a list of (file_off, len, d_ptr); every range lands at its d_ptr in one pipelined pass and
+        every block a range touches is CRC-verified whole (see verify()).  Does not move pos.  -> sum of the lengths."""
+        n = ctypes.c_int64()
+        _check(_lib.lib().cv_readv_device(self._h, self._ranges(ranges), len(ranges), ctypes.c_void_p(stream), ctypes.byref(n)))
+        return n.value
+
+    def readv_plan(self, ranges):
+        """What readv_device(ranges) executes (host-only; the d_ptr of each range is not looked at).
+        -> (spans, n_blocks, fetch_bytes): spans in file order as (block_index, block_off, len, range_index, direct); fetch_bytes = the
+        summed length of the touched blocks, which is what the read moves."""
+        arr = self._ranges(ranges)
+        ns, nb, fb = ctypes.c_int32(), ctypes.c_int64(), ctypes.c_int64()
+        _check(_lib.lib().cv_readv_plan(self._h, arr, len(ranges), None, None, None, None, None, 0, ctypes.byref(ns), ctypes.byref(nb), ctypes.byref(fb)))
+        cap = max(1, ns.value)
+        a64 = [(ctypes.c_int64 * cap)() for _ in range(3)]
+        a32 = [(ctypes.c_int32 * cap)() for _ in range(2)]
+        _check(_lib.lib().cv_readv_plan(self._h, arr, len(ranges), a64[0], a64[1], a64[2], a32[0], a32[1], cap, ctypes.byref(ns), ctypes.byref(nb),
+                                        ctypes.byref(fb)))
+        spans = [(a64[0][i], a64[1][i], a64[2][i], a32[0][i], bool(a32[1][i])) for i in range(ns.value)]
+        return spans, nb.value, fb.value
+
     def fuse_read_device(self, pos: int, size: int, d_scratch: int, d_page_base: int, page_offsets, page_size: int,
                          stream: int = 0) -> int:
         arr = (ctypes.c_uint64 * len(page_offsets))(*page_offsets)

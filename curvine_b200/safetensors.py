@@ -1,0 +1,119 @@
+"""safetensors checkpoints straight into HBM: every tensor of the file (or a named subset) in its own CUDA tensor, from ONE vectored
+device read (Reader.readv_device) in which every block the tensors touch is CRC-verified whole on the GPU.
+
+The format needs no dependency: an 8-byte little-endian header length, a JSON object mapping each tensor name to
+{"dtype", "shape", "data_offsets": [begin, end]} (offsets relative to the first byte after the header), an optional "__metadata__"
+entry, then the raw little-endian tensor bytes."""
+import json
+import struct
+from typing import Callable, Dict, Iterable, Optional, Tuple
+
+from . import fs as _fs
+
+# the safetensors reference reader refuses headers larger than this; a larger length is a corrupt or hostile file
+MAX_HEADER_BYTES = 100 << 20
+
+
+class SafetensorsError(ValueError):
+    """The file is not a well-formed safetensors file."""
+
+
+def dtypes() -> dict:
+    """safetensors dtype name -> torch dtype, for every dtype of the format this torch build has."""
+    import torch
+    m = {"F64": torch.float64, "F32": torch.float32, "F16": torch.float16, "BF16": torch.bfloat16, "I64": torch.int64, "I32": torch.int32,
+         "I16": torch.int16, "I8": torch.int8, "U8": torch.uint8, "BOOL": torch.bool, "F8_E4M3": torch.float8_e4m3fn,
+         "F8_E5M2": torch.float8_e5m2}
+    for name, attr in (("U16", "uint16"), ("U32", "uint32"), ("U64", "uint64")):
+        if hasattr(torch, attr):
+            m[name] = getattr(torch, attr)
+    return m
+
+
+def _is_int(x) -> bool:
+    return isinstance(x, int) and not isinstance(x, bool)
+
+
+def parse_header(read: Callable[[int, int], bytes], file_len: int) -> Tuple[int, Dict[str, tuple]]:
+    """Reads and validates the header of a safetensors file of `file_len` bytes; `read(off, n)` returns n bytes of the file at off.
+    -> (data_start, {name: (torch dtype, shape, begin, end)}) with begin/end relative to data_start.  Raises SafetensorsError."""
+    if file_len < 8:
+        raise SafetensorsError("file of %d bytes is too short for the 8-byte header length" % file_len)
+    (n,) = struct.unpack("<Q", read(0, 8))
+    if n > MAX_HEADER_BYTES:
+        raise SafetensorsError("header length %d exceeds the %d-byte limit" % (n, MAX_HEADER_BYTES))
+    if 8 + n > file_len:
+        raise SafetensorsError("header length %d runs past the end of a %d-byte file" % (n, file_len))
+    try:
+        header = json.loads(read(8, n).decode("utf-8"))
+    except (UnicodeDecodeError, ValueError, RecursionError) as e:
+        raise SafetensorsError("header is not valid JSON: %s" % e)
+    if not isinstance(header, dict):
+        raise SafetensorsError("header is not a JSON object")
+    data_start, data_len = 8 + n, file_len - 8 - n
+    table = dtypes()
+    out = {}
+    for name, ent in header.items():
+        if name == "__metadata__":
+            continue
+        if not isinstance(ent, dict):
+            raise SafetensorsError("%s: entry is not an object" % name)
+        dt, shape, offs = ent.get("dtype"), ent.get("shape"), ent.get("data_offsets")
+        if dt not in table:
+            raise SafetensorsError("%s: unknown dtype %r" % (name, dt))
+        if not isinstance(shape, list) or not all(_is_int(d) and d >= 0 for d in shape):
+            raise SafetensorsError("%s: shape %r is not a list of non-negative integers" % (name, shape))
+        if not isinstance(offs, list) or len(offs) != 2 or not all(_is_int(o) for o in offs):
+            raise SafetensorsError("%s: data_offsets %r is not a pair of integers" % (name, offs))
+        begin, end = offs
+        if not 0 <= begin <= end <= data_len:
+            raise SafetensorsError("%s: data_offsets [%d, %d) lie outside the %d-byte data section" % (name, begin, end, data_len))
+        count = 1
+        for d in shape:
+            count *= d
+        if count * table[dt].itemsize != end - begin:
+            raise SafetensorsError("%s: shape %r of %s needs %d bytes, data_offsets hold %d" % (name, shape, dt, count * table[dt].itemsize, end - begin))
+        out[name] = (table[dt], tuple(shape), begin, end)
+    spans = sorted((b, e, name) for name, (_, _, b, e) in out.items() if e > b)
+    for (_, e0, n0), (b1, _, n1) in zip(spans, spans[1:]):
+        if b1 < e0:
+            raise SafetensorsError("tensors %s and %s overlap in the data section" % (n0, n1))
+    return data_start, out
+
+
+def load_file(fs: "_fs.CurvineFileSystem", path: str, device=None, names: Optional[Iterable[str]] = None,
+              verify: bool = True) -> Dict[str, "object"]:
+    """The tensors of safetensors file `path` (all of them, or those in `names`) as tensors on `device` (default: the current CUDA
+    device).  One vectored read moves them: blocks that no selected tensor touches are not fetched, and every touched block is
+    CRC-verified whole, including the bytes of unselected neighbours that share it.  Raises IOError when a block fails verification
+    and `verify` is set, SafetensorsError for a malformed header, KeyError for a name the file does not hold."""
+    import torch
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    r = fs.open(path)
+    try:
+        def read(off, n):
+            r.seek(off)
+            b = r.read_full(n)
+            if len(b) != n:
+                raise SafetensorsError("short read of the header: %d of %d bytes" % (len(b), n))
+            return b
+
+        data_start, entries = parse_header(read, r.len())
+        selected = list(entries) if names is None else list(dict.fromkeys(names))
+        for name in selected:
+            if name not in entries:
+                raise KeyError("%s holds no tensor named %r" % (path, name))
+        out, ranges = {}, []
+        for name in selected:
+            dtype, shape, begin, end = entries[name]
+            t = torch.empty(shape, dtype=dtype, device=dev)
+            out[name] = t
+            if end > begin:
+                ranges.append((data_start + begin, end - begin, t.data_ptr()))
+        r.readv_device(ranges, torch.cuda.current_stream(dev).cuda_stream)
+        _, bad, _ = r.verify()
+        if verify and bad:
+            raise IOError("%d blocks of %s failed CRC verification" % (bad, path))
+        return out
+    finally:
+        r.complete()

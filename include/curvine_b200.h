@@ -19,7 +19,7 @@
  *   cv_fuse_read                 Reader::fuse_read                         reader.rs:101-124
  *   cv_seek / cv_pos / cv_len    Reader::seek / pos / len                  reader.rs:23-48, fs_reader.rs:109-126
  *   cv_close_reader              Reader::complete + drop                   java_abi.rs:157-166
- *   cv_read_device, cv_read_device_sharded, cv_read_many_device, cv_verify, cv_fuse_read_device
+ *   cv_read_device, cv_read_device_sharded, cv_read_many_device, cv_readv_device, cv_verify, cv_fuse_read_device
  *                                the CUDA counterpart the north_star adds behind the same reader handle
  *                                (no reference counterpart: the reference has no GPU code)
  * The cv_worker_* and cv_synth_* entry points are the test/bench fixture (the analogue of the reference's
@@ -114,6 +114,25 @@ int64_t cv_read_many_device(cv_fs* fs, const char* const* paths, int32_t n, void
  * at file_off[i], is len[i] bytes long and lands at dst_off[i] = i * block_size.  Arrays may be NULL; cap = their length. */
 int64_t cv_shard_plan(cv_reader* r, int32_t rank, int32_t world, int64_t* block_index, int64_t* file_off, int64_t* len,
                       int64_t* dst_off, int32_t cap, int32_t* n, int64_t* total_bytes);
+/* Vectored device read: n byte ranges of the reader's file -> n device destinations in one pipelined pass, ordered on `stream`.
+ * Ranges may come in any order, must lie inside the file and must not overlap each other in the file; len == 0 ranges do nothing.
+ * Destinations are device memory on [b200] device, any alignment.  Every block a range touches is fetched once and its CRC is
+ * compared with the manifest over the WHOLE block, bytes no range wants included; the results accumulate into cv_verify like any
+ * device read (n_verified counts each touched block with a manifest CRC once).  A block one range covers whole lands in place;
+ * every other touched block is fetched whole into device staging (bounded, reused in rounds) and its spans are delivered from
+ * there by the K3 gather kernel.  Does not move pos.  *nbytes = sum of len.  Malformed input is an error (cv_last_error), never a crash. */
+typedef struct CvRange {
+    int64_t file_off;
+    int64_t len;
+    void* d_dst;
+} CvRange;
+int64_t cv_readv_device(cv_reader* r, const CvRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes);
+/* The plan cv_readv_device executes (host-only, no GPU needed; d_dst is not looked at), one entry per span: for i < *n_spans,
+ * bytes [block_off[i], block_off[i] + len[i]) of block block_index[i] go to range range_index[i]; direct[i] = 1 when the block lands
+ * in place (one range covers it whole), 0 when it goes through the staging.  Spans come in file order.  *n_blocks = touched blocks,
+ * *fetch_bytes = their summed length (what the read moves over PCIe).  Arrays may be NULL; cap = their length. */
+int64_t cv_readv_plan(cv_reader* r, const CvRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len,
+                      int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes);
 /* FUSE-shaped device read: seek(pos), read len bytes into HBM scratch, then scatter them into n_pages page
  * buffers (d_page_base + page_offsets[i], page_size each; last one partial) with the K3 gather kernel. */
 int64_t cv_fuse_read_device(cv_reader* r, int64_t pos, int64_t len, void* d_scratch, void* d_page_base,
