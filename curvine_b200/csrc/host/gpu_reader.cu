@@ -3,22 +3,17 @@
 #include <cuda_runtime.h>
 #include <errno.h>
 #include <fcntl.h>
-#include <sched.h>
-#include <sys/mman.h>
 #include <sys/stat.h>
 #include <unistd.h>
 
 #include <algorithm>
-#include <deque>
-#include <list>
-#include <set>
-
 #include <fstream>
 
 #include "../../../include/curvine_b200_kernels.h"
 #include "block_store.h"
 #include "gds.h"
 #include "net.h"
+#include "reg_cache.h"
 
 namespace cv {
 
@@ -32,448 +27,6 @@ namespace cv {
         int e_ = (x);                                                                               \
         if (e_ != 0) return Err::io(str_printf("%s: %s", #x, cudaGetErrorString(cudaError_t(e_)))); \
     } while (0)
-
-// ------------------------------------------------------------------ registered mem-tier mappings (zero-copy ingest)
-//
-// A mem-tier block file lives in tmpfs page-cache pages.  Instead of pread()ing it into a pinned slot (one CPU copy
-// per byte), map the block files of one copy group back to back into a reserved VA range, cudaHostRegister the range
-// once, and let the copy engine DMA straight out of the page cache.  Mappings are cached (LRU by bytes, never more than
-// `register_cache` bytes registered through the cache) and revalidated by (inode, size, mtime) on every use; block files
-// are write-once in Curvine.
-// Admission is scan-resistant: a new mapping only displaces mappings that nobody is using AND that have not been used for
-// `register_min_age` (default 5 s); otherwise the newcomer is not cached (its group keeps going through the pinned ring).
-// With plain LRU a sequential re-read of a file larger than the cache finds every group evicted just before it gets there
-// -- 0 hits while paying registration every pass; with this rule the first cache-full of groups stays registered and a
-// cyclic scan hits cache/working-set of the time, while a working set that moved away ages out after register_min_age.
-struct RegMapping {
-    std::string key;
-    uint8_t* base = nullptr;
-    size_t bytes = 0;     // registered extent (page-rounded)
-    std::vector<uint64_t> stamps;  // inode, size, mtime_ns per member file
-    bool registered = false;
-    double last_used = 0;  // now_sec() of the last find() hit or the insertion (under RegCache's lock)
-    ~RegMapping() {
-        if (registered) cudaHostUnregister(base);
-        if (base) munmap(base, bytes);
-    }
-};
-
-class RegCache {
-   public:
-    size_t capacity = 0;   // bytes; 0 disables caching (mappings live for one call)
-    double min_age_sec = 5.0;  // a mapping used more recently than this is not displaced by a newcomer
-    std::shared_ptr<RegMapping> find(const std::string& key, const std::vector<uint64_t>& stamps) {
-        std::shared_ptr<RegMapping> stale;  // destroyed (unregistered, unmapped) outside the lock
-        std::lock_guard<std::mutex> lk(mu_);
-        auto it = map_.find(key);
-        if (it == map_.end()) return nullptr;
-        if (it->second->second->stamps != stamps) {  // file replaced: drop the stale mapping
-            stale = it->second->second;
-            bytes_ -= stale->bytes;
-            lru_.erase(it->second);
-            map_.erase(it);
-            return nullptr;
-        }
-        lru_.splice(lru_.begin(), lru_, it->second);
-        it->second->second->last_used = now_sec();
-        hits++;
-        return it->second->second;
-    }
-    // -> true when the mapping was admitted.  A rejected mapping stays valid for the caller's own use and goes away with it.
-    bool insert(const std::shared_ptr<RegMapping>& m) {
-        std::vector<std::shared_ptr<RegMapping>> evicted;  // destroyed outside the lock
-        std::lock_guard<std::mutex> lk(mu_);
-        if (capacity == 0 || m->bytes > capacity) return false;
-        auto dup = map_.find(m->key);
-        if (dup != map_.end()) {  // same group registered twice (two contexts' worth of threads raced): the newer one wins
-            bytes_ -= dup->second->second->bytes;
-            evicted.push_back(dup->second->second);
-            lru_.erase(dup->second);
-            map_.erase(dup);
-        }
-        const double now = now_sec();
-        // make room from the cold end; stop at the first entry that is in use or still young
-        while (bytes_ + m->bytes > capacity && !lru_.empty()) {
-            auto& back = lru_.back();
-            if (back.second.use_count() > 1 || now - back.second->last_used < min_age_sec) break;
-            bytes_ -= back.second->bytes;
-            evicted.push_back(back.second);
-            map_.erase(back.first);
-            lru_.pop_back();
-        }
-        if (bytes_ + m->bytes > capacity) {
-            rejected++;
-            return false;
-        }
-        m->last_used = now;
-        lru_.emplace_front(m->key, m);
-        map_[m->key] = lru_.begin();
-        bytes_ += m->bytes;
-        return true;
-    }
-    // would insert() admit a mapping of `bytes` right now?  (asked BEFORE paying for mmap + cudaHostRegister)
-    bool can_admit(size_t bytes) {
-        std::lock_guard<std::mutex> lk(mu_);
-        if (capacity == 0 || bytes > capacity) return false;
-        size_t room = capacity - std::min(capacity, bytes_);
-        const double now = now_sec();
-        for (auto it = lru_.rbegin(); room < bytes && it != lru_.rend(); ++it) {
-            if (it->second.use_count() > 1 || now - it->second->last_used < min_age_sec) break;
-            room += it->second->bytes;
-        }
-        return room >= bytes;
-    }
-    void clear() {
-        std::lock_guard<std::mutex> lk(mu_);
-        map_.clear();
-        lru_.clear();
-        bytes_ = 0;
-    }
-    size_t bytes() {
-        std::lock_guard<std::mutex> lk(mu_);
-        return bytes_;
-    }
-    std::atomic<uint64_t> hits{0}, misses{0}, rejected{0};
-
-   private:
-    std::mutex mu_;
-    std::list<std::pair<std::string, std::shared_ptr<RegMapping>>> lru_;
-    std::unordered_map<std::string, std::list<std::pair<std::string, std::shared_ptr<RegMapping>>>::iterator> map_;
-    size_t bytes_ = 0;
-};
-
-// Map `paths` (lens[i] bytes each; all but the last a multiple of the page size) contiguously and register the range.
-static Err map_and_register(const std::vector<std::string>& paths, const std::vector<int64_t>& lens, std::shared_ptr<RegMapping>* out,
-                            std::vector<uint64_t>* stamps_out) {
-    const size_t page = 4096;
-    size_t total = 0;
-    for (size_t i = 0; i < paths.size(); i++) {
-        if (i + 1 < paths.size() && lens[i] % static_cast<int64_t>(page)) return Err::common("block length is not page aligned");
-        total += (static_cast<size_t>(lens[i]) + page - 1) / page * page;
-    }
-    std::shared_ptr<RegMapping> m(new RegMapping());
-    void* base = mmap(nullptr, total, PROT_NONE, MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
-    if (base == MAP_FAILED) return Err::io(str_printf("mmap reserve: %s", strerror(errno)));
-    m->base = static_cast<uint8_t*>(base), m->bytes = total;
-    size_t off = 0;
-    for (size_t i = 0; i < paths.size(); i++) {
-        // cudaHostRegister needs a writable shared mapping here (cudaHostRegisterReadOnly is not supported on this
-        // platform); nothing ever writes through it.  Read-only block files fall back to the pinned ring.
-        const int fd = ::open(paths[i].c_str(), O_RDWR | O_CLOEXEC);
-        if (fd < 0) return Err(kUnsupported, str_printf("open %s read-write: %s", paths[i].c_str(), strerror(errno)));
-        struct stat st;
-        fstat(fd, &st);
-        if (st.st_size < lens[i]) {
-            ::close(fd);
-            return Err::io("block file shorter than the block length");
-        }
-        m->stamps.push_back(static_cast<uint64_t>(st.st_ino)), m->stamps.push_back(static_cast<uint64_t>(st.st_size));
-        m->stamps.push_back(static_cast<uint64_t>(st.st_mtim.tv_sec) * 1000000000ull + static_cast<uint64_t>(st.st_mtim.tv_nsec));
-        const size_t span = (static_cast<size_t>(lens[i]) + page - 1) / page * page;
-        void* p = mmap(m->base + off, span, PROT_READ | PROT_WRITE, MAP_SHARED | MAP_FIXED | MAP_POPULATE, fd, 0);
-        ::close(fd);
-        if (p == MAP_FAILED) return Err::io(str_printf("mmap %s: %s", paths[i].c_str(), strerror(errno)));
-        off += span;
-    }
-    cudaError_t e = cudaHostRegister(m->base, total, cudaHostRegisterDefault);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        return Err(kUnsupported, str_printf("cudaHostRegister(%zu): %s", total, cudaGetErrorString(e)));
-    }
-    m->registered = true;
-    *stamps_out = m->stamps;
-    *out = std::move(m);
-    return Err::ok();
-}
-
-static bool stat_stamps(const std::vector<std::string>& paths, std::vector<uint64_t>* stamps) {
-    stamps->clear();
-    for (const auto& p : paths) {
-        struct stat st;
-        if (stat(p.c_str(), &st) != 0) return false;
-        stamps->push_back(static_cast<uint64_t>(st.st_ino)), stamps->push_back(static_cast<uint64_t>(st.st_size));
-        stamps->push_back(static_cast<uint64_t>(st.st_mtim.tv_sec) * 1000000000ull + static_cast<uint64_t>(st.st_mtim.tv_nsec));
-    }
-    return true;
-}
-
-// Background registration: a cache miss does not stall the read.  The foreground moves the group through the pinned
-// ring right away (cold pass at ring speed) while a few registrar threads mmap + cudaHostRegister the same files so that
-// the NEXT pass over them is zero-copy.  cudaHostRegister pins 4 KiB pages at a few GB/s per thread and
-// serialises with copy enqueues inside the driver, so by default (`register_when_idle`) the registrar threads yield to
-// reads in flight: `hold` counts them, and a registrar only starts a new group while it is zero (or while a caller is
-// blocked in drain()).
-class Registrar {
-   public:
-    struct Job {
-        std::string key;
-        std::vector<std::string> paths;
-        std::vector<int64_t> lens;
-    };
-    void start(int threads, int device, RegCache* cache, std::vector<int> cpus, const std::atomic<int>* hold) {
-        device_ = device, cache_ = cache, cpus_ = std::move(cpus), hold_ = hold;
-        for (int t = 0; t < threads; t++) threads_.emplace_back([this] { loop(); });
-    }
-    void submit(Job j) {
-        std::lock_guard<std::mutex> lk(mu_);
-        if (stop_ || unsupported.load() || !pending_keys_.insert(j.key).second) return;
-        q_.push_back(std::move(j));
-        cv_.notify_one();
-    }
-    void stop() {
-        {
-            std::lock_guard<std::mutex> lk(mu_);
-            stop_ = true;
-            q_.clear();
-            cv_.notify_all();
-        }
-        for (auto& t : threads_) t.join();
-        threads_.clear();
-    }
-    void drain() {  // wait until the queue is empty and no registration is in flight
-        std::unique_lock<std::mutex> lk(mu_);
-        draining_++;
-        idle_cv_.wait(lk, [&] { return (q_.empty() && busy_ == 0) || stop_; });
-        draining_--;
-    }
-    size_t backlog() {
-        std::lock_guard<std::mutex> lk(mu_);
-        return q_.size() + static_cast<size_t>(busy_);
-    }
-    std::atomic<bool> unsupported{false};
-    std::atomic<uint64_t> registered{0};
-
-   private:
-    void loop() {
-        if (!cpus_.empty()) {
-            cpu_set_t set;
-            CPU_ZERO(&set);
-            for (int c : cpus_) CPU_SET(c, &set);
-            sched_setaffinity(0, sizeof(set), &set);
-        }
-        cudaSetDevice(device_);
-        for (;;) {
-            Job j;
-            {
-                std::unique_lock<std::mutex> lk(mu_);
-                cv_.wait(lk, [&] { return stop_ || !q_.empty(); });
-                if (stop_) return;
-                if (hold_ && hold_->load(std::memory_order_acquire) > 0 && draining_ == 0) {  // a read is in flight: stay out of its way
-                    lk.unlock();
-                    usleep(300);
-                    continue;
-                }
-                j = std::move(q_.front());
-                q_.pop_front();
-                busy_++;
-            }
-            std::shared_ptr<RegMapping> m;
-            std::vector<uint64_t> stamps;
-            size_t job_bytes = 0;
-            for (int64_t l : j.lens) job_bytes += (static_cast<size_t>(l) + 4095) / 4096 * 4096;
-            Err e = cache_->can_admit(job_bytes) ? map_and_register(j.paths, j.lens, &m, &stamps) : Err(kCommon, "registration cache is full");
-            if (!e) {
-                m->key = j.key;
-                if (cache_->insert(m)) registered++;
-            } else if (e.kind == kUnsupported) {
-                unsupported.store(true);
-            }
-            std::lock_guard<std::mutex> lk(mu_);
-            pending_keys_.erase(j.key);
-            busy_--;
-            if (q_.empty() && busy_ == 0) idle_cv_.notify_all();
-        }
-    }
-    int device_ = 0;
-    RegCache* cache_ = nullptr;
-    std::vector<int> cpus_;
-    std::vector<std::thread> threads_;
-    std::mutex mu_;
-    std::condition_variable cv_, idle_cv_;
-    std::deque<Job> q_;
-    std::set<std::string> pending_keys_;
-    int busy_ = 0, draining_ = 0;
-    bool stop_ = false;
-    const std::atomic<int>* hold_ = nullptr;
-};
-
-// ------------------------------------------------------------------ mem-arena segments (pinned once, off the read path)
-//
-// An arena-backed worker (arena.h) keeps every mem-tier block as an extent of a few large tmpfs segment files.  A segment is
-// mapped and cudaHostRegister'ed ONCE per context -- in the background from the first device read on for the dirs named in
-// `[b200] arena_preregister`, on demand for any other segment an Open names -- and stays pinned until the context closes.
-// From then on every block in it, whatever file it belongs to and whenever it was written, is DMA'd straight out of the
-// segment: no per-file or per-block client state, so the first read of a file runs at the same rate as a re-read.
-// Registration is sliced (`arena_register_slice`) so that all registrar threads pin one segment together.
-struct ArenaSeg {
-    std::string path;
-    uint8_t* base = nullptr;
-    size_t bytes = 0, slice = 0;
-    uint64_t ino = 0;
-    std::vector<uint8_t> slice_registered;
-    std::mutex mu;
-    std::condition_variable cv;
-    size_t slices_left = 0;
-    bool done = false;
-    Err err;
-    ~ArenaSeg() {
-        if (base) mprotect(base, bytes, PROT_READ | PROT_WRITE);
-        for (size_t i = 0; i < slice_registered.size(); i++)
-            if (slice_registered[i]) cudaHostUnregister(base + i * slice);
-        if (base) munmap(base, bytes);
-    }
-};
-
-class ArenaSegs {
-   public:
-    std::atomic<uint64_t> dma_jobs{0}, dma_bytes{0};  // block jobs / bytes moved straight out of a pinned segment
-    std::atomic<bool> unsupported{false};             // cudaHostRegister refuses these mappings: arena blocks go through the ring
-    double register_sec = 0;                          // wall time from the first slice queued to the last one pinned (under mu_)
-
-    void start(int threads, int device, std::vector<int> cpus, size_t slice) {
-        device_ = device, cpus_ = std::move(cpus), slice_ = std::max<size_t>(slice, 2 << 20) & ~size_t(4095);
-        for (int t = 0; t < std::max(1, threads); t++) threads_.emplace_back([this] { loop(); });
-    }
-    void stop() {
-        {
-            std::lock_guard<std::mutex> lk(mu_);
-            stop_ = true;
-            q_.clear();
-            cv_.notify_all();
-        }
-        for (auto& t : threads_) t.join();
-        threads_.clear();
-        std::lock_guard<std::mutex> lk(mu_);
-        segs_.clear();
-        retired_.clear();
-    }
-    // Every seg_* file under <data_dir>/<cluster_id>/arena is queued for mapping + pinning.  Returns immediately.
-    void preregister_dir(const std::string& arena_dir) {
-        for (int k = 0;; k++) {
-            const std::string p = str_printf("%s/seg_%04d", arena_dir.c_str(), k);
-            struct stat st;
-            if (stat(p.c_str(), &st) != 0) break;
-            std::shared_ptr<ArenaSeg> seg;
-            begin(p, &seg);
-        }
-    }
-    // The pinned mapping of segment `path` (blocks until it is fully registered; starts the registration if nobody has).
-    Err get(const std::string& path, std::shared_ptr<ArenaSeg>* out) {
-        std::shared_ptr<ArenaSeg> seg;
-        CV_RETURN_IF_ERR(begin(path, &seg));
-        std::unique_lock<std::mutex> lk(seg->mu);
-        seg->cv.wait(lk, [&] { return seg->done; });
-        if (seg->err) return seg->err;
-        *out = std::move(seg);
-        return Err::ok();
-    }
-    void drain() {  // wait until everything queued so far is pinned
-        std::vector<std::shared_ptr<ArenaSeg>> all;
-        {
-            std::lock_guard<std::mutex> lk(mu_);
-            for (auto& kv : segs_) all.push_back(kv.second);
-        }
-        for (auto& seg : all) {
-            std::unique_lock<std::mutex> lk(seg->mu);
-            seg->cv.wait(lk, [&] { return seg->done; });
-        }
-    }
-    void stats(uint64_t* n_segs, uint64_t* bytes, double* sec) {
-        std::lock_guard<std::mutex> lk(mu_);
-        *n_segs = segs_.size(), *bytes = 0, *sec = register_sec;
-        for (auto& kv : segs_) *bytes += kv.second->err ? 0 : kv.second->bytes;
-    }
-
-   private:
-    Err begin(const std::string& path, std::shared_ptr<ArenaSeg>* out) {
-        struct stat st;
-        if (stat(path.c_str(), &st) != 0) return Err::io(str_printf("arena segment %s: %s", path.c_str(), strerror(errno)));
-        std::lock_guard<std::mutex> lk(mu_);
-        auto it = segs_.find(path);
-        if (it != segs_.end() && it->second->ino == static_cast<uint64_t>(st.st_ino) && it->second->bytes == static_cast<size_t>(st.st_size)) {
-            *out = it->second;
-            return Err::ok();
-        }
-        if (it != segs_.end()) retired_.push_back(it->second);  // the file was replaced (worker restarted on a fresh dir): copies may still be in flight
-        if (unsupported.load()) return Err(kUnsupported, "cudaHostRegister of arena segments is not supported here");
-        std::shared_ptr<ArenaSeg> seg(new ArenaSeg());
-        seg->path = path, seg->bytes = static_cast<size_t>(st.st_size), seg->ino = static_cast<uint64_t>(st.st_ino), seg->slice = slice_;
-        // cudaHostRegister needs a writable shared mapping (cudaHostRegisterReadOnly is refused on this platform); the mapping is
-        // write-protected again as soon as it is pinned
-        const int fd = ::open(path.c_str(), O_RDWR | O_CLOEXEC);
-        if (fd < 0) return Err(kUnsupported, str_printf("open %s read-write: %s", path.c_str(), strerror(errno)));
-        void* m = mmap(nullptr, seg->bytes, PROT_READ | PROT_WRITE, MAP_SHARED, fd, 0);
-        ::close(fd);
-        if (m == MAP_FAILED) return Err::io(str_printf("mmap %s: %s", path.c_str(), strerror(errno)));
-        seg->base = static_cast<uint8_t*>(m);
-        const size_t n = (seg->bytes + slice_ - 1) / slice_;
-        seg->slice_registered.assign(n, 0);
-        seg->slices_left = n;
-        if (busy_ == 0 && q_.empty()) t_first_ = now_sec();
-        for (size_t i = 0; i < n; i++) q_.emplace_back(seg, i);
-        segs_[path] = seg;
-        cv_.notify_all();
-        *out = std::move(seg);
-        return Err::ok();
-    }
-    void loop() {
-        if (!cpus_.empty()) {
-            cpu_set_t set;
-            CPU_ZERO(&set);
-            for (int c : cpus_) CPU_SET(c, &set);
-            sched_setaffinity(0, sizeof(set), &set);
-        }
-        cudaSetDevice(device_);
-        for (;;) {
-            std::pair<std::shared_ptr<ArenaSeg>, size_t> job;
-            {
-                std::unique_lock<std::mutex> lk(mu_);
-                cv_.wait(lk, [&] { return stop_ || !q_.empty(); });
-                if (stop_) return;
-                job = std::move(q_.front());
-                q_.pop_front();
-                busy_++;
-            }
-            ArenaSeg& seg = *job.first;
-            const size_t off = job.second * seg.slice, len = std::min(seg.slice, seg.bytes - off);
-#ifdef MADV_POPULATE_WRITE
-            // map the slice's (already allocated) tmpfs pages in bulk first: the page-by-page faults cudaHostRegister would
-            // otherwise take on a fresh mapping are what made pinning 3x slower than on the mapping that created the pages
-            madvise(seg.base + off, len, MADV_POPULATE_WRITE);
-#endif
-            const cudaError_t ce = cudaHostRegister(seg.base + off, len, cudaHostRegisterDefault);
-            if (ce != cudaSuccess) cudaGetLastError();
-            bool last = false;
-            {
-                std::lock_guard<std::mutex> lk(seg.mu);
-                if (ce == cudaSuccess) seg.slice_registered[job.second] = 1;
-                else if (!seg.err) seg.err = Err(kUnsupported, str_printf("cudaHostRegister(%s + %zu, %zu): %s", seg.path.c_str(), off, len, cudaGetErrorString(ce)));
-                last = --seg.slices_left == 0;
-                if (last) {
-                    if (!seg.err) mprotect(seg.base, seg.bytes, PROT_READ);  // pinned pages stay DMA-able; nothing in this process can scribble on them
-                    else unsupported.store(true);
-                    seg.done = true;
-                    seg.cv.notify_all();
-                }
-            }
-            std::lock_guard<std::mutex> lk(mu_);
-            busy_--;
-            if (busy_ == 0 && q_.empty()) register_sec += now_sec() - t_first_;
-        }
-    }
-    int device_ = 0;
-    size_t slice_ = 256 << 20;
-    std::vector<int> cpus_;
-    std::vector<std::thread> threads_;
-    std::mutex mu_;
-    std::condition_variable cv_;
-    std::deque<std::pair<std::shared_ptr<ArenaSeg>, size_t>> q_;
-    std::unordered_map<std::string, std::shared_ptr<ArenaSeg>> segs_;
-    std::vector<std::shared_ptr<ArenaSeg>> retired_;
-    int busy_ = 0;
-    double t_first_ = 0;
-    bool stop_ = false;
-};
 
 // ------------------------------------------------------------------ GpuIngest: ring + streams
 
@@ -592,16 +145,8 @@ class GpuIngest {
         return Err::ok();
     }
 
-    void bind_thread() const {
-        if (cpus.empty()) return;
-        cpu_set_t set;
-        CPU_ZERO(&set);
-        for (int c : cpus) CPU_SET(c, &set);
-        sched_setaffinity(0, sizeof(set), &set);
-    }
-
     Err ensure(size_t need_slot_bytes, bool framed) {
-        need_slot_bytes = (need_slot_bytes + 4095) & ~size_t(4095);
+        need_slot_bytes = page_up(need_slot_bytes);
         if (need_slot_bytes > slot_bytes) {
             CU_TRY(cudaDeviceSynchronize());
             if (pinned) cudaFreeHost(pinned);
@@ -613,7 +158,7 @@ class GpuIngest {
             Err err;
             const double t0 = now_sec();
             std::thread t([&] {
-                bind_thread();
+                bind_cpus(cpus);
                 cudaSetDevice(device);
                 cudaError_t e = cudaHostAlloc(&pinned, slot_bytes * nslots, cudaHostAllocDefault);
                 if (e != cudaSuccess) err = Err::io(str_printf("cudaHostAlloc(%zu): %s", slot_bytes * nslots, cudaGetErrorString(e)));
@@ -862,12 +407,25 @@ static inline void backoff_wait(F cond) {
 
 enum FetchMode { kFetchShortCircuit = 0, kFetchFramedVerbatim = 1 };
 
-// Fetch one job's bytes into `slot`.
-//   short-circuit    payload only (pread of the block file the worker named)
-//   framed verbatim  the response stream exactly as received: 22-byte prefixes + payloads (unpacked on the GPU by K2, which
-//                    also clips the last chunk of a range that stops short of the block end)
-static Err fetch_job(FsContext* ctx, const LocatedBlock& lb, int64_t block_off, int64_t n, FetchMode mode, int64_t chunk, uint8_t* slot,
-                     std::unique_ptr<BlockClient>* conn, int64_t* req_id_out, size_t* wire_bytes) {
+// n bytes of the file at `path` from file_off -> buf
+static Err pread_full(const std::string& path, int64_t file_off, uint8_t* buf, int64_t n) {
+    const int fd = ::open(path.c_str(), O_RDONLY | O_CLOEXEC);
+    if (fd < 0) return Err::io(str_printf("open %s: %s", path.c_str(), strerror(errno)));
+    Err e;
+    for (int64_t got = 0; got < n && !e;) {
+        const ssize_t r = pread(fd, buf + got, static_cast<size_t>(n - got), file_off + got);
+        if (r < 0 && errno == EINTR) continue;
+        if (r <= 0) e = Err::io(str_printf("read block file: %s", r == 0 ? "unexpected eof" : strerror(errno)));
+        else got += r;
+    }
+    ::close(fd);
+    return e;
+}
+
+// fn(connection) on each replica of `lb` in turn until one succeeds (a pooled `conn` to the replica is reused while it is healthy);
+// -> the last error when none did.
+template <typename F>
+static Err for_each_replica(FsContext* ctx, const LocatedBlock& lb, std::unique_ptr<BlockClient>* conn, F fn) {
     Err last = ctx->no_available_worker(lb.locs);
     for (const WorkerAddress& loc : lb.locs) {
         if (!*conn || !((*conn)->addr() == loc) || (*conn)->broken) {
@@ -875,102 +433,76 @@ static Err fetch_job(FsContext* ctx, const LocatedBlock& lb, int64_t block_off, 
             last = ctx->acquire_read(loc, conn);
             if (last) continue;
         }
-        BlockClient* c = conn->get();
+        last = fn(conn->get());
+        if (!last) return Err::ok();
+    }
+    return last;
+}
+
+// Open(short_circuit=true) on connection `c`: the worker names the block file (and, for an arena block, the extent inside it)
+static Err open_on(FsContext* ctx, BlockClient* c, const LocatedBlock& lb, int64_t block_off, int64_t req_id, BlockReadResponse* resp) {
+    CV_RETURN_IF_ERR(c->open_block(ctx->conf.client, lb.block, block_off, lb.block.len, req_id, 0, true, ctx->read_chunk_size(), resp, ctx->conf.b200.arena));
+    return resp->has_path ? Err::ok() : Err::common("read_context.path is none");
+}
+
+// Fetch one job's bytes into `slot`.
+//   short-circuit    payload only (pread of the block file the worker named)
+//   framed verbatim  the response stream exactly as received: 22-byte prefixes + payloads (unpacked on the GPU by K2, which
+//                    also clips the last chunk of a range that stops short of the block end)
+// A replica whose block file cannot be read is given up for the next one.
+static Err fetch_job(FsContext* ctx, const LocatedBlock& lb, int64_t block_off, int64_t n, FetchMode mode, int64_t chunk, uint8_t* slot,
+                     std::unique_ptr<BlockClient>* conn, int64_t* req_id_out, size_t* wire_bytes) {
+    return for_each_replica(ctx, lb, conn, [&](BlockClient* c) -> Err {
         const int64_t req_id = new_req_id();
         *req_id_out = req_id;
         BlockReadResponse resp;
-        if (mode == kFetchFramedVerbatim) {
-            // Open + every Running request + Complete in one write (the worker serves them in order, read_handler.rs:60-207).  The
-            // worker answers each Running with min(chunk, block_len - pos) bytes, so the last frame of a range that stops short of
-            // the block end carries bytes past it: they are received like the rest and clipped by K2 (CvStreamDesc.tail_clip).
-            const int64_t nfr = (n + chunk - 1) / chunk;
-            n = std::min<int64_t>(nfr * chunk, lb.block.len - block_off);  // payload bytes on the wire
-            last = c->send_block_read_pipeline(ctx->conf.client, lb.block, block_off, req_id, chunk, nfr, &resp);
-            if (last) continue;
-            uint8_t* w = slot;
-            int64_t left = n;
-            for (int64_t f = 0; f < nfr && !last; f++) {
-                last = recv_exact(c->fd(), w, kProtocolSize);
-                Protocol p;
-                if (!last) last = decode_protocol(w, &p);
-                if (last) break;
-                const int64_t want = std::min(chunk, left);
-                if (!p.is_success() || p.header_len != 0 || p.data_len != want) {
-                    // error response (or an unexpected chunk): drain this frame, report it, drop the connection
-                    std::string body(static_cast<size_t>(p.header_len + p.data_len), '\0');
-                    if (!body.empty() && recv_exact(c->fd(), &body[0], body.size())) c->broken = true;
-                    last = p.is_success() ? Err::common(str_printf("unexpected chunk length %d, expected %lld", p.data_len, (long long)want))
-                                          : decode_error_body(reinterpret_cast<const uint8_t*>(body.data()) + p.header_len, static_cast<size_t>(p.data_len));
-                    break;
-                }
-                last = recv_exact(c->fd(), w + kProtocolSize, static_cast<size_t>(want));
-                w += kProtocolSize + want, left -= want;
-            }
-            if (last) {
-                c->broken = true;  // responses of the remaining pipelined requests may still be in flight
-                continue;
-            }
-            *wire_bytes = static_cast<size_t>(w - slot);
-            return Err::ok();  // the Complete went out with the rest; its answer is consumed in front of this connection's next request
-        }
-        const int64_t open_chunk = ctx->read_chunk_size();
-        last = c->open_block(ctx->conf.client, lb.block, block_off, lb.block.len, req_id, 0, true, open_chunk, &resp, ctx->conf.b200.arena);
-        if (last) continue;
-        int32_t seq = 0;
-        const int64_t base_off = resp.has_arena ? resp.arena_off : 0;  // arena block: an extent inside the segment file
         if (mode == kFetchShortCircuit) {
-            if (!resp.has_path) {
-                last = Err::common("read_context.path is none");
-                continue;
-            }
-            const int fd = ::open(resp.path.c_str(), O_RDONLY | O_CLOEXEC);
-            if (fd < 0) {
-                last = Err::io(str_printf("open %s: %s", resp.path.c_str(), strerror(errno)));
-                continue;
-            }
-            int64_t got = 0;
-            while (got < n) {
-                const ssize_t r = pread(fd, slot + got, static_cast<size_t>(n - got), base_off + block_off + got);
-                if (r < 0 && errno == EINTR) continue;
-                if (r <= 0) {
-                    last = Err::io(str_printf("read block file: %s", r == 0 ? "unexpected eof" : strerror(errno)));
-                    break;
-                }
-                got += r;
-            }
-            ::close(fd);
-            if (got < n) continue;
+            CV_RETURN_IF_ERR(open_on(ctx, c, lb, block_off, req_id, &resp));
+            CV_RETURN_IF_ERR(pread_full(resp.path, (resp.has_arena ? resp.arena_off : 0) + block_off, slot, n));  // arena block: an extent of the segment file
             *wire_bytes = static_cast<size_t>(n);
+            return c->read_commit_deferred(lb.block, req_id, 1);  // its answer is consumed in front of this connection's next request
         }
-        last = c->read_commit_deferred(lb.block, req_id, seq + 1);  // its answer is consumed in front of this connection's next request
-        if (last) continue;
-        return Err::ok();
-    }
-    return last;
+        // Open + every Running request + Complete in one write (the worker serves them in order, read_handler.rs:60-207).  The
+        // worker answers each Running with min(chunk, block_len - pos) bytes, so the last frame of a range that stops short of
+        // the block end carries bytes past it: they are received like the rest and clipped by K2 (CvStreamDesc.tail_clip).
+        const int64_t nfr = (n + chunk - 1) / chunk;
+        int64_t left = std::min<int64_t>(nfr * chunk, lb.block.len - block_off);  // payload bytes on the wire
+        CV_RETURN_IF_ERR(c->send_block_read_pipeline(ctx->conf.client, lb.block, block_off, req_id, chunk, nfr, &resp));
+        uint8_t* w = slot;
+        Err e;
+        for (int64_t f = 0; f < nfr && !e; f++) {
+            e = recv_exact(c->fd(), w, kProtocolSize);
+            Protocol p;
+            if (!e) e = decode_protocol(w, &p);
+            if (e) break;
+            const int64_t want = std::min(chunk, left);
+            if (!p.is_success() || p.header_len != 0 || p.data_len != want) {
+                // error response (or an unexpected chunk): drain this frame, report it, drop the connection
+                std::string body(static_cast<size_t>(p.header_len + p.data_len), '\0');
+                if (!body.empty() && recv_exact(c->fd(), &body[0], body.size())) c->broken = true;
+                e = p.is_success() ? Err::common(str_printf("unexpected chunk length %d, expected %lld", p.data_len, (long long)want))
+                                   : decode_error_body(reinterpret_cast<const uint8_t*>(body.data()) + p.header_len, static_cast<size_t>(p.data_len));
+                break;
+            }
+            e = recv_exact(c->fd(), w + kProtocolSize, static_cast<size_t>(want));
+            w += kProtocolSize + want, left -= want;
+        }
+        if (e) {
+            c->broken = true;  // responses of the remaining pipelined requests may still be in flight
+            return e;
+        }
+        *wire_bytes = static_cast<size_t>(w - slot);
+        return Err::ok();  // the Complete went out with the rest; its answer is consumed in front of this connection's next request
+    });
 }
 
 // Open(short_circuit=true) on the first replica that answers; returns the block file path.
 static Err open_short_circuit(FsContext* ctx, const LocatedBlock& lb, int64_t block_off, std::unique_ptr<BlockClient>* conn, int64_t* req_id,
                               BlockReadResponse* out) {
-    Err last = ctx->no_available_worker(lb.locs);
-    for (const WorkerAddress& loc : lb.locs) {
-        if (!*conn || !((*conn)->addr() == loc) || (*conn)->broken) {
-            if (*conn) ctx->release(std::move(*conn));
-            last = ctx->acquire_read(loc, conn);
-            if (last) continue;
-        }
+    return for_each_replica(ctx, lb, conn, [&](BlockClient* c) {
         *req_id = new_req_id();
-        BlockReadResponse resp;
-        last = (*conn)->open_block(ctx->conf.client, lb.block, block_off, lb.block.len, *req_id, 0, true, ctx->read_chunk_size(), &resp, ctx->conf.b200.arena);
-        if (last) continue;
-        if (!resp.has_path) {
-            last = Err::common("read_context.path is none");
-            continue;
-        }
-        *out = resp;
-        return Err::ok();
-    }
-    return last;
+        return open_on(ctx, c, lb, block_off, *req_id, out);
+    });
 }
 
 // Pull the last call's per-block CRCs / mismatch count / frame flags (already copied to the pinned mirror on vstream).
@@ -1019,6 +551,425 @@ static Err check_device_dst(const void* p, int device) {
     return Err::ok();
 }
 
+enum JobMode : uint8_t { kPlain = 0, kFramed = 1, kHole = 3 };
+
+// Layout of the per-call device tables (shared by all readers of the context) and of their pinned host image:
+//   off[J] len[J] expect[J] skip[J] | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F] | segs[n_segs]
+// off .. skip are uploaded before the fetch starts; crc .. ferr are the results copied back.
+struct TableLayout {
+    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, o_segs = 0, bytes = 0;
+    TableLayout() = default;
+    TableLayout(size_t j, size_t f, size_t n_segs) : J(j), F(f) {
+        auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
+        o_len = up(8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_crc = up(o_skip + J);
+        o_streams = up(o_crc + 4 * res_words()), o_fdesc = up(o_streams + sizeof(CvStreamDesc) * J);
+        o_segs = up(o_fdesc + sizeof(CvFrameDesc) * F), bytes = up(o_segs + sizeof(CvSeg) * n_segs);
+    }
+    size_t res_words() const { return J + 4 + F; }
+    uint64_t* off(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t); }
+    uint64_t* len(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t + o_len); }
+    uint32_t* expect(uint8_t* t) const { return reinterpret_cast<uint32_t*>(t + o_exp); }
+    uint8_t* skip(uint8_t* t) const { return t + o_skip; }
+    uint32_t* crc(uint8_t* t) const { return reinterpret_cast<uint32_t*>(t + o_crc); }
+    uint32_t* ferr(uint8_t* t) const { return crc(t) + J + 4; }
+    CvStreamDesc* streams(uint8_t* t) const { return reinterpret_cast<CvStreamDesc*>(t + o_streams); }
+    CvFrameDesc* fdesc(uint8_t* t) const { return reinterpret_cast<CvFrameDesc*>(t + o_fdesc); }
+    CvSeg* segs(uint8_t* t) const { return reinterpret_cast<CvSeg*>(t + o_segs); }
+};
+
+// What one run_jobs call does, decided before any CUDA call.
+struct GpuFsReader::CallPlan {
+    std::vector<uint8_t> mode;             // JobMode per job
+    bool call_framed = false;              // a block without a local replica (or short_circuit off): every job runs framed
+    bool any_verbatim = false;             // some job is received verbatim (framed) and unpacked by K2
+    std::vector<int64_t> wire_payload;     // framed jobs: payload bytes the worker sends (>= n when the range stops short of the block end)
+    std::vector<uint32_t> first_frame;     // [J + 1]: first frame of each job
+    size_t F = 0;                          // frames in the call
+    size_t need_slot = 0;                  // pinned-slot bytes the largest job needs
+    int64_t chunk = 0;                     // framed chunk size
+    size_t k = 1, NG = 0, NS = 0;          // jobs per copy group, copy groups in the call, super-slots in the ring
+    size_t vgroups = 1, B = 1;             // copy groups per verify launch, and the jobs they hold
+    std::vector<uint8_t> group_verbatim;   // per copy group: holds a framed job
+    int T_threads = 1;                     // fetch workers
+    TableLayout tl;
+};
+
+Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, CallPlan* out) const {
+    CallPlan& P = *out;
+    const B200Conf& bc = ctx_->conf.b200;
+    const size_t J = jobs.size();
+    P.chunk = std::min<int64_t>(std::max<int64_t>(bc.gpu_chunk_size, 4096), kMaxDataSize);
+    // Short-circuit (the reference default for a same-host worker, client_conf.rs:339) only when every block of this call has a local
+    // replica; otherwise the whole call runs framed (any worker serves those).
+    P.mode.assign(J, kPlain);
+    for (size_t j = 0; j < J; j++) {
+        const LocatedBlock& lb = *jobs[j].lb;
+        if (lb.locs.empty()) {
+            if (!lb.block.has_alloc_opts) return ctx_->no_available_worker(lb.locs);
+            P.mode[j] = kHole;
+            continue;
+        }
+        bool local = false;
+        for (const auto& a : lb.locs) local |= ctx_->is_local_worker(a);
+        if (!(ctx_->conf.client.short_circuit && local)) P.call_framed = true;
+    }
+    P.first_frame.assign(J + 1, 0);
+    P.wire_payload.assign(J, 0);
+    for (size_t j = 0; j < J; j++) {
+        P.first_frame[j] = static_cast<uint32_t>(P.F);
+        size_t bytes = static_cast<size_t>(jobs[j].n);
+        if (P.mode[j] != kHole && P.call_framed) {
+            // every framed job is received verbatim and unpacked by K2; a range that stops short of its block's end gets the
+            // worker's whole last chunk and K2 clips it (CvStreamDesc.tail_clip) -- no host-side unpacking anywhere
+            P.mode[j] = kFramed;
+            const int64_t nfr = (jobs[j].n + P.chunk - 1) / P.chunk;
+            P.wire_payload[j] = std::min<int64_t>(nfr * P.chunk, jobs[j].lb->block.len - jobs[j].block_off);
+            bytes = static_cast<size_t>(P.wire_payload[j] + nfr * kProtocolSize);
+            P.F += static_cast<size_t>(nfr);
+            P.any_verbatim = true;
+        }
+        P.need_slot = std::max(P.need_slot, bytes);
+    }
+    P.first_frame[J] = static_cast<uint32_t>(P.F);
+    // copy groups: k consecutive jobs share one super-slot and, when they are contiguous, one cudaMemcpyAsync
+    P.k = static_cast<size_t>(std::max(1, std::min(bc.copy_group, ing_->nslots / 4)));
+    P.NG = (J + P.k - 1) / P.k;
+    P.NS = static_cast<size_t>(ing_->nslots) / P.k;
+    P.vgroups = std::max<size_t>(1, (static_cast<size_t>(std::max(1, bc.verify_batch)) + P.k - 1) / P.k);
+    P.B = P.vgroups * P.k;
+    P.group_verbatim.assign(P.NG, 0);
+    for (size_t j = 0; j < J; j++) P.group_verbatim[j / P.k] |= P.mode[j] == kFramed;
+    P.T_threads = static_cast<int>(std::min<size_t>(static_cast<size_t>(std::max(1, bc.fetch_threads)), P.NG));
+    P.tl = TableLayout(J, P.F, n_segs);
+    return Err::ok();
+}
+
+namespace {
+
+// Host-to-device copies of (dst, src, len) pieces on one stream.  A piece that continues the previous one in the source AND in the
+// destination extends it, so one cudaMemcpyAsync moves both -- except across a register slice of an arena segment: a copy never spans
+// two separately registered slices.
+struct H2D {
+    cudaStream_t cs;
+    uint64_t* counted;  // bytes enqueued (the reader's h2d_bytes)
+    uint8_t* dst = nullptr;
+    const uint8_t* src = nullptr;
+    size_t len = 0;
+    bool pending = false;
+    const ArenaSeg* seg = nullptr;  // the pending piece's source lies in this segment
+    cudaError_t ce = cudaSuccess;
+
+    H2D(cudaStream_t s, uint64_t* c) : cs(s), counted(c) {}
+    bool ok() const { return ce == cudaSuccess; }
+    void add(uint8_t* d, const uint8_t* s, size_t n, const ArenaSeg* sg = nullptr) {
+        if (pending && sg == seg && d == dst + len && s == src + len) {
+            len += n;
+            return;
+        }
+        flush();
+        dst = d, src = s, len = n, seg = sg, pending = true;
+    }
+    void flush() {
+        if (!pending || !ok()) return;
+        for (size_t done = 0; done < len && ok();) {
+            size_t piece = len - done;
+            if (seg) {
+                const size_t in_seg = static_cast<size_t>(src - seg->base) + done;
+                piece = std::min(piece, (in_seg / seg->slice + 1) * seg->slice - in_seg);
+            }
+            ce = cudaMemcpyAsync(dst + done, src + done, piece, cudaMemcpyHostToDevice, cs);
+            done += piece;
+        }
+        *counted += len;
+        pending = false;
+    }
+    Err finish() {
+        flush();
+        return ok() ? Err::ok() : Err::io(str_printf("H2D enqueue: %s", cudaGetErrorString(ce)));
+    }
+};
+
+}  // namespace
+
+// One run_jobs call in flight: the fetch workers, the per-call state they share with the verifier, and the ingest paths a copy group
+// can take.  Each path returns Err::ok() when the group's copies are enqueued, kUnsupported when the group must go to the next path
+// (GDS -> registered mappings / arena -> pinned ring), or the error that fails the call.
+struct GpuFsReader::Call {
+    struct Group {
+        size_t g, ss, j0, j1;  // copy group, its super-slot, its jobs [j0, j1)
+        int t;                 // fetch worker
+        cudaStream_t cs;
+    };
+    GpuFsReader& r;
+    GpuIngest& G;
+    const std::vector<Job>& jobs;
+    const CallPlan& P;
+    uint8_t* d_dst;
+    std::atomic<size_t> next_group{0};
+    std::atomic<bool> abort{false};
+    std::mutex err_mu, held_mu;
+    Err err;
+    std::vector<std::atomic<int>> copied;
+    std::vector<std::atomic<int64_t>> released;  // per super-slot: last copy group whose release event is recorded
+    std::vector<int64_t> req_ids;
+    std::atomic<bool> use_mapped, use_gds;
+    std::atomic<uint64_t> gds_bytes{0};
+    std::vector<double> fetch_sec;
+    std::vector<uint64_t> h2d;
+    std::once_flag ring_once;
+    Err ring_err;
+
+    Call(GpuFsReader& reader, const std::vector<Job>& js, const CallPlan& plan, uint8_t* dst)
+        : r(reader), G(*reader.ing_), jobs(js), P(plan), d_dst(dst), copied(plan.NG), released(plan.NS), req_ids(js.size(), 0),
+          fetch_sec(static_cast<size_t>(plan.T_threads), 0.0), h2d(static_cast<size_t>(plan.T_threads), 0) {
+        const B200Conf& bc = r.ctx_->conf.b200;
+        for (auto& c : copied) c.store(0);
+        for (auto& x : released) x.store(-1);
+        use_mapped.store(bc.zero_copy);
+        bool any_disk = false;  // cuFile is probed only by a read that has disk-tier blocks
+        for (size_t j = 0; j < jobs.size() && !any_disk; j++) any_disk = jobs[j].lb->block.storage_type != kStorageMem;
+        use_gds.store(!P.call_framed && bc.gds != 0 && any_disk && gds_info().available);
+    }
+    void fail(const Err& e) {
+        std::lock_guard<std::mutex> lk(err_mu);
+        if (!err) err = e;
+        abort.store(true);
+    }
+    // the pinned ring (and the device staging ring for verbatim frames) is only materialised when a group needs it: the zero-copy
+    // path never touches it
+    Err ensure_ring() {
+        std::call_once(ring_once, [&] { ring_err = G.ensure(P.need_slot, P.any_verbatim); });
+        return ring_err;
+    }
+    uint8_t* slot_base(const Group& gr) const { return G.pinned + gr.ss * P.k * G.slot_bytes; }
+
+    void worker(int t, bool own_thread) {
+        if (own_thread) bind_cpus(G.cpus);  // an inline call (single copy group: small reads) must not re-pin the caller
+        cudaSetDevice(G.device);
+        cudaStream_t cs = G.copy_streams[static_cast<size_t>(t) % G.copy_streams.size()];
+        std::unique_ptr<BlockClient> conn;
+        for (;;) {
+            const size_t g = next_group.fetch_add(1);
+            if (g >= P.NG || abort.load()) break;
+            const Group gr{g, g % P.NS, g * P.k, std::min(jobs.size(), g * P.k + P.k), t, cs};
+            if (!wait_slot(gr)) break;
+            bool all_plain = true, all_disk = true;
+            for (size_t j = gr.j0; j < gr.j1; j++) {
+                all_plain = all_plain && P.mode[j] == kPlain;
+                all_disk = all_disk && jobs[j].lb->block.storage_type != kStorageMem;
+            }
+            Err e(kUnsupported, "");  // kUnsupported: the group goes to the next path
+            if (all_plain && all_disk && use_gds.load(std::memory_order_relaxed)) {
+                e = fetch_group_gds(gr, &conn);
+                if (e.kind == kUnsupported) use_gds.store(false);  // this file system / this box cannot do it: the next path redoes the group
+            }
+            if (e.kind == kUnsupported && all_plain && use_mapped.load(std::memory_order_relaxed)) {
+                e = fetch_group_mapped(gr, &conn);
+                if (e.kind == kUnsupported) use_mapped.store(false);  // cannot register file mappings here: the pinned ring takes over
+            }
+            if (e.kind == kUnsupported) e = fetch_group_ring(gr, &conn);
+            if (!publish(gr, e)) break;
+        }
+        if (conn) {
+            // multi-group reads: settle the deferred Completes here (their answers are long in); a single-group read (the
+            // latency path, C5) parks the connection with its last answer outstanding and the next request consumes it
+            if (P.NG > 1) conn->drain_pending();
+            r.ctx_->release(std::move(conn));
+        }
+    }
+
+    // A super-slot serves every NS-th group: wait until its previous tenant has been released, then for that tenant's copies (or,
+    // for a verbatim group, its K2) to finish with the slot.
+    bool wait_slot(const Group& gr) {
+        if (gr.g < P.NS) return true;
+        const int64_t want = static_cast<int64_t>(gr.g - P.NS);
+        backoff_wait([&] { return released[gr.ss].load(std::memory_order_acquire) >= want || abort.load(); });
+        if (abort.load()) return false;
+        cudaEventSynchronize(P.group_verbatim[gr.g - P.NS] ? G.free_ev[gr.ss] : G.copy_ev[gr.ss]);
+        return true;
+    }
+
+    // Hand the group to the verifier once its copies are enqueued.  A verbatim group's super-slot is released by the verifier after
+    // K2 has unpacked it; every other group's as soon as its copy event is recorded.
+    bool publish(const Group& gr, const Err& e) {
+        const cudaError_t ce = e ? cudaSuccess : cudaEventRecord(G.copy_ev[gr.ss], gr.cs);
+        if (e || ce != cudaSuccess) {
+            fail(e ? e : Err::io(str_printf("event record: %s", cudaGetErrorString(ce))));
+            return false;
+        }
+        if (!P.group_verbatim[gr.g]) released[gr.ss].store(static_cast<int64_t>(gr.g), std::memory_order_release);
+        copied[gr.g].store(1, std::memory_order_release);
+        return true;
+    }
+
+    // GPUDirect Storage: blocks of a disk tier go file -> HBM by cuFileRead, no host ring
+    Err fetch_group_gds(const Group& gr, std::unique_ptr<BlockClient>* conn) {
+        const double t0 = now_sec();
+        backoff_wait([&] { return cudaEventQuery(G.entry_ev) != cudaErrorNotReady; });  // cuFile knows nothing of the caller's stream
+        Err e;
+        for (size_t j = gr.j0; j < gr.j1 && !e; j++) {
+            const Job& job = jobs[j];
+            BlockReadResponse resp;
+            int64_t rid = 0;
+            e = open_short_circuit(r.ctx_, *job.lb, job.block_off, conn, &rid, &resp);
+            if (!e) e = gds_read(resp.path, d_dst + job.dst_off, job.n, (resp.has_arena ? resp.arena_off : 0) + job.block_off);
+            if (!e) e = (*conn)->read_commit_deferred(job.lb->block, rid, 1);
+            if (!e) gds_bytes += static_cast<uint64_t>(job.n);
+        }
+        fetch_sec[static_cast<size_t>(gr.t)] += now_sec() - t0;
+        return e;
+    }
+
+    // Zero-copy: DMA out of the mem arena's pinned segments, or out of registered mmaps of the block files.  Groups whose mappings
+    // are not ready (or cannot be pinned) are pread out of the block files into the ring.
+    Err fetch_group_mapped(const Group& gr, std::unique_ptr<BlockClient>* conn) {
+        const double t0 = now_sec();
+        const size_t n = gr.j1 - gr.j0;
+        std::vector<std::string> paths(n);
+        std::vector<int64_t> lens(n), rids(n), base_offs(n, 0);
+        size_t n_arena = 0;
+        Err e;
+        for (size_t i = 0; i < n && !e; i++) {
+            const Job& job = jobs[gr.j0 + i];
+            BlockReadResponse resp;
+            e = open_short_circuit(r.ctx_, *job.lb, job.block_off, conn, &rids[i], &resp);
+            paths[i] = resp.path, lens[i] = job.lb->block.len;
+            if (resp.has_arena) base_offs[i] = resp.arena_off, n_arena++;
+        }
+        bool via_ring = n_arena > 0;  // arena extents (mixed group, or segments that cannot be pinned): pread out of the segment file
+        if (!e && n_arena == n && !G.arena.unsupported.load(std::memory_order_relaxed)) {
+            e = fetch_arena(gr, paths, base_offs, rids, conn);
+            if (e.kind != kUnsupported) {
+                fetch_sec[static_cast<size_t>(gr.t)] += now_sec() - t0;
+                return e;
+            }
+            e = Err::ok();  // segments cannot be pinned here: the group goes through the ring
+        }
+        std::shared_ptr<RegMapping> m;
+        if (!e && !via_ring) e = find_mapping(paths, lens, &m, &via_ring);
+        H2D q(gr.cs, &h2d[static_cast<size_t>(gr.t)]);
+        if (!e && via_ring) {
+            e = ensure_ring();
+            if (!e) e = fill_ring(gr, q, [&](size_t j, uint8_t* at, size_t* wire) {
+                    *wire = static_cast<size_t>(jobs[j].n);
+                    return pread_full(paths[j - gr.j0], base_offs[j - gr.j0] + jobs[j].block_off, at, jobs[j].n);
+                });
+        } else if (!e) {
+            size_t moff = 0;  // the group's block files lie back to back in the mapping, each page-rounded
+            for (size_t i = 0; i < n; i++) {
+                const Job& job = jobs[gr.j0 + i];
+                q.add(d_dst + job.dst_off, m->base + moff + job.block_off, static_cast<size_t>(job.n));
+                moff += page_up(static_cast<size_t>(lens[i]));
+            }
+            std::lock_guard<std::mutex> lk(held_mu);
+            r.held_maps_.push_back(m);
+        }
+        const Err copy_err = e ? Err::ok() : q.finish();
+        for (size_t j = gr.j0; j < gr.j1 && !e; j++) e = (*conn)->read_commit(jobs[j].lb->block, rids[j - gr.j0], 1);
+        fetch_sec[static_cast<size_t>(gr.t)] += now_sec() - t0;
+        return e ? e : copy_err;
+    }
+
+    // Every block of the group is an extent of an arena segment this context pinned once.  kUnsupported: a segment cannot be pinned.
+    Err fetch_arena(const Group& gr, const std::vector<std::string>& paths, const std::vector<int64_t>& base_offs, const std::vector<int64_t>& rids,
+                    std::unique_ptr<BlockClient>* conn) {
+        std::vector<std::shared_ptr<ArenaSeg>> segs(paths.size());
+        for (size_t i = 0; i < paths.size(); i++) {
+            const Job& job = jobs[gr.j0 + i];
+            if (i > 0 && paths[i] == paths[i - 1]) segs[i] = segs[i - 1];
+            else CV_RETURN_IF_ERR(G.arena.get(paths[i], &segs[i]));
+            if (static_cast<size_t>(base_offs[i] + job.block_off + job.n) > segs[i]->bytes) return Err::io("arena extent lies outside its segment");
+        }
+        H2D q(gr.cs, &h2d[static_cast<size_t>(gr.t)]);
+        for (size_t i = 0; i < paths.size(); i++) {
+            const Job& job = jobs[gr.j0 + i];
+            q.add(d_dst + job.dst_off, segs[i]->base + base_offs[i] + job.block_off, static_cast<size_t>(job.n), segs[i].get());
+        }
+        const Err copy_err = q.finish();
+        Err e;
+        for (size_t j = gr.j0; j < gr.j1 && !e; j++) e = (*conn)->read_commit_deferred(jobs[j].lb->block, rids[j - gr.j0], 1);
+        if (e || copy_err) return e ? e : copy_err;
+        G.arena.dma_jobs += gr.j1 - gr.j0;
+        for (size_t j = gr.j0; j < gr.j1; j++) G.arena.dma_bytes += static_cast<uint64_t>(jobs[j].n);
+        return Err::ok();
+    }
+
+    // The registered mapping of the group's block files: a cache hit, or registered now when the cache does the registration inline.
+    // *via_ring when the group goes through the ring this time (cache full of young mappings, or registration left to the background).
+    Err find_mapping(const std::vector<std::string>& paths, const std::vector<int64_t>& lens, std::shared_ptr<RegMapping>* m, bool* via_ring) {
+        std::string key;
+        for (const auto& p : paths) key += p, key += '|';
+        std::vector<uint64_t> stamps;
+        if (stat_stamps(paths, &stamps)) *m = G.reg.find(key, stamps);
+        if (*m) return Err::ok();
+        G.reg.misses++;
+        if (G.registrar.unsupported.load()) return Err(kUnsupported, "cudaHostRegister of file mappings is not supported here");
+        size_t group_bytes = 0;
+        for (int64_t l : lens) group_bytes += page_up(static_cast<size_t>(l));
+        if (G.reg.capacity > 0 && !G.reg.can_admit(group_bytes)) {
+            // the cache is full of mappings in use or used moments ago (a scan larger than the cache): registering this group would be
+            // paid for and thrown away -- it goes through the ring, now and next time
+            G.reg.rejected++;
+            *via_ring = true;
+        } else if (G.register_inline) {
+            CV_RETURN_IF_ERR(map_and_register(paths, lens, m, &stamps));
+            (*m)->key = key;
+            G.reg.insert(*m);
+        } else {  // cold group: register it in the background for the next pass, move it through the ring now
+            G.registrar.submit(Registrar::Job{key, paths, lens});
+            *via_ring = true;
+        }
+        return Err::ok();
+    }
+
+    // The pinned ring: each job is fetched into the group's super-slot and copied from there (holes are zero-filled on the device).
+    Err fetch_group_ring(const Group& gr, std::unique_ptr<BlockClient>* conn) {
+        CV_RETURN_IF_ERR(ensure_ring());
+        H2D q(gr.cs, &h2d[static_cast<size_t>(gr.t)]);
+        CV_RETURN_IF_ERR(fill_ring(gr, q, [&](size_t j, uint8_t* at, size_t* wire) {
+            const Job& job = jobs[j];
+            const double t0 = now_sec();
+            const FetchMode fm = P.mode[j] == kPlain ? kFetchShortCircuit : kFetchFramedVerbatim;
+            Err e = fetch_job(r.ctx_, *job.lb, job.block_off, job.n, fm, P.chunk, at, conn, &req_ids[j], wire);
+            fetch_sec[static_cast<size_t>(gr.t)] += now_sec() - t0;
+            return e ? e.ctx(str_printf("block %lld", (long long)job.lb->block.id)) : e;
+        }));
+        return q.finish();
+    }
+
+    // Slot layout of a ring group: when its jobs are all plain, back to back in the destination and fit into the super-slot, they
+    // mirror the destination layout there and one copy moves the group; otherwise each job has a slot (and a copy) of its own.
+    // fetch(j, at, &wire) puts job j's bytes at `at`; a verbatim group's frames go to the device staging in one copy after the last.
+    template <typename Fetch>
+    Err fill_ring(const Group& gr, H2D& q, Fetch fetch) {
+        const Job& first = jobs[gr.j0];
+        const Job& last = jobs[gr.j1 - 1];
+        bool mirror = static_cast<size_t>(last.dst_off + last.n - first.dst_off) <= P.k * G.slot_bytes;
+        for (size_t j = gr.j0; j < gr.j1 && mirror; j++)
+            mirror = P.mode[j] == kPlain && (j == gr.j0 || jobs[j].dst_off == jobs[j - 1].dst_off + jobs[j - 1].n);
+        uint8_t* hs = slot_base(gr);
+        size_t wire_extent = 0;
+        for (size_t j = gr.j0; j < gr.j1 && q.ok(); j++) {
+            const Job& job = jobs[j];
+            if (P.mode[j] == kHole) {
+                q.ce = cudaMemsetAsync(d_dst + job.dst_off, 0, static_cast<size_t>(job.n), gr.cs);  // block_reader_hole.rs:69-79
+                continue;
+            }
+            const size_t at = mirror ? static_cast<size_t>(job.dst_off - first.dst_off) : (j - gr.j0) * G.slot_bytes;
+            size_t wire = 0;
+            CV_RETURN_IF_ERR(fetch(j, hs + at, &wire));
+            if (P.mode[j] == kFramed) {
+                wire_extent = at + wire;
+            } else {
+                q.add(d_dst + job.dst_off, hs + at, wire);
+                if (!mirror) q.flush();
+            }
+        }
+        if (wire_extent) q.add(G.d_stage + (hs - G.pinned), hs, wire_extent);
+        return Err::ok();
+    }
+};
+
 Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* user_stream, const Scatter* pages) {
     const size_t J = jobs.size();
     if (J == 0) return Err::ok();
@@ -1040,88 +991,29 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     for (auto cs : G.copy_streams) CU_TRY(cudaStreamWaitEvent(cs, G.entry_ev, 0));
     CU_TRY(cudaStreamWaitEvent(G.vstream, G.entry_ev, 0));
     const B200Conf& bc = ctx_->conf.b200;
-    const ClientConf& cc = ctx_->conf.client;
     const int poly = bc.verify_poly ? 1 : 0;
-    const int64_t chunk = std::min<int64_t>(std::max<int64_t>(bc.gpu_chunk_size, 4096), kMaxDataSize);
-
-    // ---- per-job mode.  Short-circuit (the reference default for a same-host worker, client_conf.rs:339) only when
-    // every block of this call has a local replica; otherwise the whole call runs framed (any worker serves those).
-    enum : uint8_t { kPlain = 0, kFramed = 1, kHole = 3 };
-    std::vector<uint8_t> mode(J, kPlain);
-    bool call_framed = false;
-    for (size_t j = 0; j < J; j++) {
-        const LocatedBlock& lb = (*jobs[j].lb);
-        if (lb.locs.empty()) {
-            if (!lb.block.has_alloc_opts) return ctx_->no_available_worker(lb.locs);
-            mode[j] = kHole;
-            continue;
-        }
-        bool local = false;
-        for (const auto& a : lb.locs) local |= ctx_->is_local_worker(a);
-        if (!(cc.short_circuit && local)) call_framed = true;
-    }
-    size_t need_slot = 0, F = 0;
-    std::vector<uint32_t> first_frame(J + 1, 0);
-    bool any_verbatim = false;
-    std::vector<int64_t> wire_payload(J, 0);  // framed jobs: payload bytes the worker sends (>= n when the range stops short of the block end)
-    for (size_t j = 0; j < J; j++) {
-        first_frame[j] = static_cast<uint32_t>(F);
-        size_t bytes = static_cast<size_t>(jobs[j].n);
-        if (mode[j] != kHole && call_framed) {
-            // every framed job is received verbatim and unpacked by K2; a range that stops short of its block's end gets the
-            // worker's whole last chunk and K2 clips it (CvStreamDesc.tail_clip) -- no host-side unpacking anywhere
-            mode[j] = kFramed;
-            const int64_t nfr = (jobs[j].n + chunk - 1) / chunk;
-            wire_payload[j] = std::min<int64_t>(nfr * chunk, (*jobs[j].lb).block.len - jobs[j].block_off);
-            bytes = static_cast<size_t>(wire_payload[j] + nfr * kProtocolSize);
-            F += static_cast<size_t>(nfr);
-            any_verbatim = true;
-        }
-        need_slot = std::max(need_slot, bytes);
-    }
-    first_frame[J] = static_cast<uint32_t>(F);
-    // the pinned ring (and the device staging ring for verbatim frames) is only materialised when a group needs it:
-    // the zero-copy path never touches it
-    std::once_flag ring_once;
-    Err ring_err;
-    auto ensure_ring = [&]() -> Err {
-        std::call_once(ring_once, [&] { ring_err = G.ensure(need_slot, any_verbatim); });
-        return ring_err;
-    };
-    if (!(bc.zero_copy && !call_framed)) CV_RETURN_IF_ERR(ensure_ring());
-
-    // ---- copy groups: k consecutive jobs share one super-slot and, when they are contiguous, one cudaMemcpyAsync
-    const size_t k = static_cast<size_t>(std::max(1, std::min(bc.copy_group, G.nslots / 4)));
-    const size_t NG = (J + k - 1) / k;                    // copy groups in this call
-    const size_t NS = static_cast<size_t>(G.nslots) / k;  // super-slots in the ring
-    const size_t vgroups = std::max<size_t>(1, (static_cast<size_t>(std::max(1, bc.verify_batch)) + k - 1) / k);  // copy groups per verify launch
-    const size_t B = vgroups * k;
-
-    // ---- device tables (shared by all readers of this context): off[J] len[J] | expect[J] crc[J] nbad[4] ferr[F] | streams[J] fdesc[F]
-    auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
-    const size_t o_off = 0, o_len = up(o_off + 8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_crc = up(o_skip + J);
-    const size_t res_words = J + 4 + F;
-    const size_t o_streams = up(o_crc + 4 * res_words), o_fdesc = up(o_streams + sizeof(CvStreamDesc) * J);
     const size_t n_segs = pages ? pages->segs.size() : 0;
-    const size_t o_segs = up(o_fdesc + sizeof(CvFrameDesc) * F);
-    const size_t tables_bytes = up(o_segs + sizeof(CvSeg) * n_segs);
-    CV_RETURN_IF_ERR(G.ensure_tables(tables_bytes, 4 * res_words));
+
+    CallPlan P;
+    CV_RETURN_IF_ERR(plan_call(jobs, n_segs, &P));
+    Call c(*this, jobs, P, d_dst);
+    if (!(bc.zero_copy && !P.call_framed)) CV_RETURN_IF_ERR(c.ensure_ring());
+
+    // ---- tables.  The host image is pinned, owned by the context, and rewritten only after the previous call's results were
+    // harvested (its uploads have long executed by then).
+    const TableLayout& tl = P.tl;
+    CV_RETURN_IF_ERR(G.ensure_tables(tl.bytes, 4 * tl.res_words()));
     uint8_t* T = G.d_tables;
-    // host image of off/len/expect/skip (+ the stream descriptors): pinned, owned by the context, rewritten only after the
-    // previous call's results were harvested (its uploads have long executed by then)
     uint8_t* h = G.h_tables;
-    uint64_t* h_off = reinterpret_cast<uint64_t*>(&h[o_off]);
-    uint64_t* h_len = reinterpret_cast<uint64_t*>(&h[o_len]);
-    uint32_t* h_exp = reinterpret_cast<uint32_t*>(&h[o_exp]);
-    uint8_t* h_skip = &h[o_skip];
+    const uint64_t* h_len = tl.len(h);
     size_t f0 = J, f1 = 0, n_compared = 0;
     for (size_t j = 0; j < J; j++) {
-        const LocatedBlock& lb = (*jobs[j].lb);
-        h_off[j] = static_cast<uint64_t>(jobs[j].dst_off);
-        h_len[j] = static_cast<uint64_t>(jobs[j].n);
-        h_exp[j] = poly ? lb.crc32c : lb.crc32;
-        h_skip[j] = !(jobs[j].full && lb.has_crc && mode[j] != kHole);
-        if (!h_skip[j]) {
+        const LocatedBlock& lb = *jobs[j].lb;
+        tl.off(h)[j] = static_cast<uint64_t>(jobs[j].dst_off);
+        tl.len(h)[j] = static_cast<uint64_t>(jobs[j].n);
+        tl.expect(h)[j] = poly ? lb.crc32c : lb.crc32;
+        tl.skip(h)[j] = !(jobs[j].full && lb.has_crc && P.mode[j] != kHole);
+        if (!tl.skip(h)[j]) {
             f0 = std::min(f0, j), f1 = std::max(f1, j + 1);
             n_compared++;
         }
@@ -1130,408 +1022,101 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     // every whole block the manifest holds a CRC for is compared; holes, partial ranges and blocks without a manifest CRC are
     // masked out one by one (their CRCs are still computed, and summed when they lie inside [f0,f1))
     const bool compare = bc.verify && n_compared > 0;
-    CU_TRY(cudaMemcpyAsync(T, h, o_crc, cudaMemcpyHostToDevice, G.vstream));
+    CU_TRY(cudaMemcpyAsync(T, h, tl.o_crc, cudaMemcpyHostToDevice, G.vstream));
     if (n_segs) {  // the scatter's segment table rides in the same pinned image
-        CvSeg* hs = reinterpret_cast<CvSeg*>(h + o_segs);
-        memcpy(hs, pages->segs.data(), sizeof(CvSeg) * n_segs);
-        CU_TRY(cudaMemcpyAsync(T + o_segs, hs, sizeof(CvSeg) * n_segs, cudaMemcpyHostToDevice, G.vstream));
+        memcpy(tl.segs(h), pages->segs.data(), sizeof(CvSeg) * n_segs);
+        CU_TRY(cudaMemcpyAsync(tl.segs(T), tl.segs(h), sizeof(CvSeg) * n_segs, cudaMemcpyHostToDevice, G.vstream));
     }
-    CU_TRY(cudaMemsetAsync(T + o_crc, 0, 4 * res_words, G.vstream));
-    CvStreamDesc* sd = reinterpret_cast<CvStreamDesc*>(h + o_streams);
-    if (any_verbatim) {
+    CU_TRY(cudaMemsetAsync(tl.crc(T), 0, 4 * tl.res_words(), G.vstream));
+    CvStreamDesc* sd = tl.streams(h);
+    if (P.any_verbatim) {
         for (size_t j = 0; j < J; j++) {
             CvStreamDesc& d = sd[j];
             memset(&d, 0, sizeof(d));
-            const size_t ss = (j / k) % NS;
-            d.wire_off = (ss * k + j % k) * G.slot_bytes, d.dst_off = h_off[j], d.block_len = mode[j] == kFramed ? static_cast<uint64_t>(wire_payload[j]) : 0;
-            d.tail_clip = mode[j] == kFramed ? static_cast<uint32_t>(wire_payload[j] - jobs[j].n) : 0;
-            d.chunk_size = static_cast<uint32_t>(chunk), d.first_seq_id = 1, d.block = static_cast<uint32_t>(j % B);
-            d.first_frame = first_frame[j], d.code = kCodeReadBlock, d.status = 0x03;
+            const size_t ss = (j / P.k) % P.NS;
+            d.wire_off = (ss * P.k + j % P.k) * G.slot_bytes, d.dst_off = tl.off(h)[j];
+            d.block_len = P.mode[j] == kFramed ? static_cast<uint64_t>(P.wire_payload[j]) : 0;
+            d.tail_clip = P.mode[j] == kFramed ? static_cast<uint32_t>(P.wire_payload[j] - jobs[j].n) : 0;
+            d.chunk_size = static_cast<uint32_t>(P.chunk), d.first_seq_id = 1, d.block = static_cast<uint32_t>(j % P.B);
+            d.first_frame = P.first_frame[j], d.code = kCodeReadBlock, d.status = 0x03;
         }
     }
 
-    // ---- fetch threads
-    struct Shared {
-        std::atomic<size_t> next_group{0};
-        std::atomic<bool> abort{false};
-        std::mutex err_mu;
-        Err err;
-        void fail(const Err& e) {
-            std::lock_guard<std::mutex> lk(err_mu);
-            if (!err) err = e;
-            abort.store(true);
-        }
-    } st;
-    std::vector<std::atomic<int>> copied(NG);
-    std::vector<std::atomic<int64_t>> released(NS);  // per super-slot: last copy group whose release event is recorded
-    for (auto& c : copied) c.store(0);
-    for (auto& r : released) r.store(-1);
-    std::vector<uint8_t> group_verbatim(NG, 0);
-    for (size_t g = 0; g < NG; g++)
-        for (size_t j = g * k; j < std::min(J, g * k + k); j++) group_verbatim[g] |= mode[j] == kFramed;
-    std::vector<int64_t> req_ids(J, 0);
-    std::atomic<bool> use_mapped{bc.zero_copy};
-    bool any_disk = false;  // cuFile is probed only by a read that has disk-tier blocks
-    for (size_t j = 0; j < J && !any_disk; j++) any_disk = (*jobs[j].lb).block.storage_type != kStorageMem;
-    std::atomic<bool> use_gds{!call_framed && bc.gds != 0 && any_disk && gds_info().available};
-    std::atomic<uint64_t> gds_bytes{0};
-    std::mutex held_mu;
-    const int T_threads = static_cast<int>(std::min<size_t>(static_cast<size_t>(std::max(1, bc.fetch_threads)), NG));
-    std::vector<double> fetch_sec(static_cast<size_t>(T_threads), 0.0);
-    std::vector<uint64_t> h2d(static_cast<size_t>(T_threads), 0);
-    auto worker = [&](int t, bool own_thread) {
-        if (own_thread) G.bind_thread();  // an inline call (single copy group: small reads) must not re-pin the caller
-        cudaSetDevice(G.device);
-        cudaStream_t cs = G.copy_streams[static_cast<size_t>(t) % G.copy_streams.size()];
-        std::unique_ptr<BlockClient> conn;
-        for (;;) {
-            const size_t g = st.next_group.fetch_add(1);
-            if (g >= NG || st.abort.load()) break;
-            const size_t ss = g % NS, j0 = g * k, j1 = std::min(J, j0 + k);
-            if (g >= NS) {  // wait until the super-slot's previous tenant has been released, then for its event
-                const int64_t want = static_cast<int64_t>(g - NS);
-                backoff_wait([&] { return released[ss].load(std::memory_order_acquire) >= want || st.abort.load(); });
-                if (st.abort.load()) break;
-                cudaEventSynchronize(group_verbatim[g - NS] ? G.free_ev[ss] : G.copy_ev[ss]);
-            }
-            bool all_plain = true;
-            for (size_t j = j0; j < j1; j++) all_plain = all_plain && mode[j] == kPlain;
-            // ---- GPUDirect Storage: blocks of a disk tier go file -> HBM by cuFileRead, no host ring
-            bool all_disk = all_plain && use_gds.load(std::memory_order_relaxed);
-            for (size_t j = j0; j < j1 && all_disk; j++) all_disk = (*jobs[j].lb).block.storage_type != kStorageMem;
-            if (all_disk) {
-                const double t0 = now_sec();
-                Err e;
-                backoff_wait([&] { return cudaEventQuery(G.entry_ev) != cudaErrorNotReady; });  // cuFile knows nothing of the caller's stream
-                for (size_t j = j0; j < j1 && !e; j++) {
-                    BlockReadResponse resp;
-                    int64_t rid = 0;
-                    e = open_short_circuit(ctx_, (*jobs[j].lb), jobs[j].block_off, &conn, &rid, &resp);
-                    if (!e) e = gds_read(resp.path, d_dst + jobs[j].dst_off, jobs[j].n, (resp.has_arena ? resp.arena_off : 0) + jobs[j].block_off);
-                    if (!e) e = conn->read_commit_deferred((*jobs[j].lb).block, rid, 1);
-                    if (!e) gds_bytes += static_cast<uint64_t>(jobs[j].n);
-                }
-                fetch_sec[static_cast<size_t>(t)] += now_sec() - t0;
-                if (e && e.kind == kUnsupported) {
-                    use_gds.store(false);  // this file system / this box cannot do it: the pinned ring takes over (the group is redone below)
-                } else {
-                    cudaError_t ce = e ? cudaSuccess : cudaEventRecord(G.copy_ev[ss], cs);
-                    if (e || ce != cudaSuccess) {
-                        st.fail(e ? e : Err::io(str_printf("event record: %s", cudaGetErrorString(ce))));
-                        break;
-                    }
-                    released[ss].store(static_cast<int64_t>(g), std::memory_order_release);
-                    copied[g].store(1, std::memory_order_release);
-                    continue;
-                }
-            }
-            // ---- zero-copy: DMA out of registered mmaps of the block files (mem tier), no pinned-slot copy
-            if (all_plain && use_mapped.load(std::memory_order_relaxed)) {
-                const double t0 = now_sec();
-                std::vector<std::string> paths(j1 - j0);
-                std::vector<int64_t> lens(j1 - j0), rids(j1 - j0), base_offs(j1 - j0, 0);
-                Err e;
-                size_t n_arena = 0;
-                for (size_t j = j0; j < j1 && !e; j++) {
-                    const LocatedBlock& lb = (*jobs[j].lb);
-                    BlockReadResponse resp;
-                    e = open_short_circuit(ctx_, lb, jobs[j].block_off, &conn, &rids[j - j0], &resp);
-                    paths[j - j0] = resp.path, lens[j - j0] = lb.block.len;
-                    if (resp.has_arena) base_offs[j - j0] = resp.arena_off, n_arena++;
-                }
-                // ---- mem arena: every block of the group is an extent of a segment this context pinned once
-                if (!e && n_arena == j1 - j0 && !G.arena.unsupported.load(std::memory_order_relaxed)) {
-                    std::vector<std::shared_ptr<ArenaSeg>> segs(j1 - j0);
-                    for (size_t j = j0; j < j1 && !e; j++) {
-                        if (j > j0 && paths[j - j0] == paths[j - j0 - 1]) segs[j - j0] = segs[j - j0 - 1];
-                        else e = G.arena.get(paths[j - j0], &segs[j - j0]);
-                        if (!e && static_cast<size_t>(base_offs[j - j0] + jobs[j].block_off + jobs[j].n) > segs[j - j0]->bytes) e = Err::io("arena extent lies outside its segment");
-                    }
-                    if (!e) {
-                        cudaError_t ce = cudaSuccess;
-                        // one cudaMemcpyAsync per run of jobs that are back to back in the segment AND in the destination
-                        for (size_t j = j0; j < j1 && ce == cudaSuccess;) {
-                            const uint8_t* src = segs[j - j0]->base + base_offs[j - j0] + jobs[j].block_off;
-                            size_t len = static_cast<size_t>(jobs[j].n), r = j + 1;
-                            while (r < j1 && segs[r - j0] == segs[j - j0] && segs[r - j0]->base + base_offs[r - j0] + jobs[r].block_off == src + len &&
-                                   jobs[r].dst_off == jobs[j].dst_off + static_cast<int64_t>(len))
-                                len += static_cast<size_t>(jobs[r].n), r++;
-                            // a copy never spans two separately registered slices of the segment
-                            const ArenaSeg& sg = *segs[j - j0];
-                            for (size_t done = 0; done < len && ce == cudaSuccess;) {
-                                const size_t in_seg = static_cast<size_t>(src - sg.base) + done;
-                                const size_t piece = std::min(len - done, (in_seg / sg.slice + 1) * sg.slice - in_seg);
-                                ce = cudaMemcpyAsync(d_dst + jobs[j].dst_off + done, src + done, piece, cudaMemcpyHostToDevice, cs);
-                                done += piece;
-                            }
-                            h2d[static_cast<size_t>(t)] += len;
-                            j = r;
-                        }
-                        if (ce == cudaSuccess) ce = cudaEventRecord(G.copy_ev[ss], cs);
-                        for (size_t j = j0; j < j1 && !e; j++) e = conn->read_commit_deferred((*jobs[j].lb).block, rids[j - j0], 1);
-                        fetch_sec[static_cast<size_t>(t)] += now_sec() - t0;
-                        if (e || ce != cudaSuccess) {
-                            st.fail(e ? e : Err::io(str_printf("H2D enqueue: %s", cudaGetErrorString(ce))));
-                            break;
-                        }
-                        G.arena.dma_jobs += j1 - j0;
-                        for (size_t j = j0; j < j1; j++) G.arena.dma_bytes += static_cast<uint64_t>(jobs[j].n);
-                        released[ss].store(static_cast<int64_t>(g), std::memory_order_release);
-                        copied[g].store(1, std::memory_order_release);
-                        continue;
-                    }
-                    if (e.kind == kUnsupported) e = Err::ok();  // segments cannot be pinned here: the group goes through the ring below
-                }
-                std::shared_ptr<RegMapping> m;
-                bool via_ring = n_arena > 0;  // arena extents (mixed group, or segments that cannot be pinned): pread out of the segment file
-                if (!e && !via_ring) {
-                    std::string key;
-                    for (const auto& p : paths) key += p, key += '|';
-                    std::vector<uint64_t> stamps;
-                    if (stat_stamps(paths, &stamps)) m = G.reg.find(key, stamps);
-                    if (!m) G.reg.misses++;
-                    if (!m && G.registrar.unsupported.load()) e = Err(kUnsupported, "cudaHostRegister of file mappings is not supported here");
-                    if (!m && !e) {
-                        size_t group_bytes = 0;
-                        for (int64_t l : lens) group_bytes += (static_cast<size_t>(l) + 4095) / 4096 * 4096;
-                        if (G.reg.capacity > 0 && !G.reg.can_admit(group_bytes)) {
-                            // the cache is full of mappings in use or used moments ago (a scan larger than the cache): registering
-                            // this group would be paid for and thrown away -- it goes through the ring, now and next time
-                            G.reg.rejected++;
-                            via_ring = true;
-                        } else if (G.register_inline) {
-                            e = map_and_register(paths, lens, &m, &stamps);
-                            if (!e) {
-                                m->key = key;
-                                G.reg.insert(m);
-                            }
-                        } else {  // cold group: register it in the background for the next pass, move it through the ring now
-                            G.registrar.submit(Registrar::Job{key, paths, lens});
-                            via_ring = true;
-                        }
-                    }
-                }
-                cudaError_t ce = cudaSuccess;
-                if (!e && via_ring) {
-                    e = ensure_ring();
-                    uint8_t* hs = G.pinned + ss * k * G.slot_bytes;
-                    bool contiguous = true;
-                    for (size_t j = j0 + 1; j < j1; j++) contiguous = contiguous && jobs[j].dst_off == jobs[j - 1].dst_off + jobs[j - 1].n;
-                    if (contiguous && static_cast<size_t>(jobs[j1 - 1].dst_off + jobs[j1 - 1].n - jobs[j0].dst_off) > k * G.slot_bytes) contiguous = false;
-                    for (size_t j = j0; j < j1 && !e && ce == cudaSuccess; j++) {
-                        const size_t in_slot = contiguous ? static_cast<size_t>(jobs[j].dst_off - jobs[j0].dst_off) : (j - j0) * G.slot_bytes;
-                        const int fd = ::open(paths[j - j0].c_str(), O_RDONLY | O_CLOEXEC);
-                        if (fd < 0) {
-                            e = Err::io(str_printf("open %s: %s", paths[j - j0].c_str(), strerror(errno)));
-                            break;
-                        }
-                        int64_t got = 0;
-                        while (got < jobs[j].n) {
-                            const ssize_t r = pread(fd, hs + in_slot + got, static_cast<size_t>(jobs[j].n - got), base_offs[j - j0] + jobs[j].block_off + got);
-                            if (r < 0 && errno == EINTR) continue;
-                            if (r <= 0) {
-                                e = Err::io(str_printf("read block file: %s", r == 0 ? "unexpected eof" : strerror(errno)));
-                                break;
-                            }
-                            got += r;
-                        }
-                        ::close(fd);
-                        if (!e && !contiguous) {
-                            ce = cudaMemcpyAsync(d_dst + jobs[j].dst_off, hs + in_slot, static_cast<size_t>(jobs[j].n), cudaMemcpyHostToDevice, cs);
-                            h2d[static_cast<size_t>(t)] += static_cast<size_t>(jobs[j].n);
-                        }
-                    }
-                    if (!e && contiguous && ce == cudaSuccess) {
-                        const size_t extent = static_cast<size_t>(jobs[j1 - 1].dst_off + jobs[j1 - 1].n - jobs[j0].dst_off);
-                        ce = cudaMemcpyAsync(d_dst + jobs[j0].dst_off, hs, extent, cudaMemcpyHostToDevice, cs);
-                        h2d[static_cast<size_t>(t)] += extent;
-                    }
-                    if (!e && ce == cudaSuccess) ce = cudaEventRecord(G.copy_ev[ss], cs);
-                    for (size_t j = j0; j < j1 && !e; j++) e = conn->read_commit((*jobs[j].lb).block, rids[j - j0], 1);
-                } else if (!e) {
-                    // one copy when the group is whole blocks landing back to back, else one per job
-                    bool whole = true;
-                    for (size_t j = j0; j < j1; j++) {
-                        whole = whole && jobs[j].block_off == 0 && (j + 1 == j1 || jobs[j].n == lens[j - j0]);
-                        if (j > j0) whole = whole && jobs[j].dst_off == jobs[j - 1].dst_off + jobs[j - 1].n;
-                    }
-                    if (whole) {
-                        const size_t extent = static_cast<size_t>(jobs[j1 - 1].dst_off + jobs[j1 - 1].n - jobs[j0].dst_off);
-                        ce = cudaMemcpyAsync(d_dst + jobs[j0].dst_off, m->base, extent, cudaMemcpyHostToDevice, cs);
-                        h2d[static_cast<size_t>(t)] += extent;
-                    } else {
-                        size_t moff = 0;
-                        for (size_t j = j0; j < j1 && ce == cudaSuccess; j++) {
-                            ce = cudaMemcpyAsync(d_dst + jobs[j].dst_off, m->base + moff + jobs[j].block_off, static_cast<size_t>(jobs[j].n), cudaMemcpyHostToDevice, cs);
-                            h2d[static_cast<size_t>(t)] += static_cast<size_t>(jobs[j].n);
-                            moff += (static_cast<size_t>(lens[j - j0]) + 4095) / 4096 * 4096;
-                        }
-                    }
-                    if (ce == cudaSuccess) ce = cudaEventRecord(G.copy_ev[ss], cs);
-                    {
-                        std::lock_guard<std::mutex> lk(held_mu);
-                        held_maps_.push_back(m);
-                    }
-                    for (size_t j = j0; j < j1 && !e; j++) e = conn->read_commit((*jobs[j].lb).block, rids[j - j0], 1);
-                }
-                fetch_sec[static_cast<size_t>(t)] += now_sec() - t0;
-                if (e && e.kind == kUnsupported) {
-                    use_mapped.store(false);  // cannot register file mappings here: fall back to the pinned ring below
-                } else {
-                    if (e || ce != cudaSuccess) {
-                        st.fail(e ? e : Err::io(str_printf("H2D enqueue: %s", cudaGetErrorString(ce))));
-                        break;
-                    }
-                    released[ss].store(static_cast<int64_t>(g), std::memory_order_release);
-                    copied[g].store(1, std::memory_order_release);
-                    continue;
-                }
-            }
-            if (Err re = ensure_ring()) {
-                st.fail(re);
-                break;
-            }
-            uint8_t* hs = G.pinned + ss * k * G.slot_bytes;
-            uint8_t* ds = G.d_stage ? G.d_stage + ss * k * G.slot_bytes : nullptr;
-            // plain jobs mirror the destination layout inside the super-slot so that one copy moves the whole group
-            bool one_copy = !group_verbatim[g];
-            for (size_t j = j0; j < j1 && one_copy; j++) {
-                one_copy = mode[j] == kPlain;
-                if (j > j0) one_copy = one_copy && jobs[j].dst_off == jobs[j - 1].dst_off + jobs[j - 1].n;
-            }
-            if (one_copy && static_cast<size_t>(jobs[j1 - 1].dst_off + jobs[j1 - 1].n - jobs[j0].dst_off) > k * G.slot_bytes) one_copy = false;
-            cudaError_t ce = cudaSuccess;
-            size_t wire_extent = 0;
-            bool failed = false;
-            for (size_t j = j0; j < j1 && !failed; j++) {
-                const Job& job = jobs[j];
-                if (mode[j] == kHole) {
-                    ce = cudaMemsetAsync(d_dst + job.dst_off, 0, static_cast<size_t>(job.n), cs);  // block_reader_hole.rs:69-79
-                    failed = ce != cudaSuccess;
-                    continue;
-                }
-                const size_t in_slot = one_copy ? static_cast<size_t>(job.dst_off - jobs[j0].dst_off) : (j - j0) * G.slot_bytes;
-                size_t wire = 0;
-                const double t0 = now_sec();
-                const FetchMode fm = mode[j] == kPlain ? kFetchShortCircuit : kFetchFramedVerbatim;
-                Err e = fetch_job(ctx_, (*job.lb), job.block_off, job.n, fm, chunk, hs + in_slot, &conn, &req_ids[j], &wire);
-                fetch_sec[static_cast<size_t>(t)] += now_sec() - t0;
-                if (e) {
-                    st.fail(e.ctx(str_printf("block %lld", (long long)(*job.lb).block.id)));
-                    failed = true;
-                    break;
-                }
-                if (group_verbatim[g]) {
-                    if (mode[j] == kFramed) wire_extent = in_slot + wire;  // copied below in one piece
-                    else ce = cudaMemcpyAsync(d_dst + job.dst_off, hs + in_slot, wire, cudaMemcpyHostToDevice, cs), h2d[static_cast<size_t>(t)] += wire;
-                } else if (!one_copy) {
-                    ce = cudaMemcpyAsync(d_dst + job.dst_off, hs + in_slot, wire, cudaMemcpyHostToDevice, cs), h2d[static_cast<size_t>(t)] += wire;
-                }
-                failed = ce != cudaSuccess;
-            }
-            if (st.abort.load() && failed && ce == cudaSuccess) break;
-            if (!failed && group_verbatim[g] && wire_extent) {
-                ce = cudaMemcpyAsync(ds, hs, wire_extent, cudaMemcpyHostToDevice, cs);
-                h2d[static_cast<size_t>(t)] += wire_extent;
-            } else if (!failed && one_copy) {
-                const size_t extent = static_cast<size_t>(jobs[j1 - 1].dst_off + jobs[j1 - 1].n - jobs[j0].dst_off);
-                ce = cudaMemcpyAsync(d_dst + jobs[j0].dst_off, hs, extent, cudaMemcpyHostToDevice, cs);
-                h2d[static_cast<size_t>(t)] += extent;
-            }
-            if (ce == cudaSuccess && !failed) ce = cudaEventRecord(G.copy_ev[ss], cs);
-            if (ce != cudaSuccess) {
-                st.fail(Err::io(str_printf("H2D enqueue: %s", cudaGetErrorString(ce))));
-                break;
-            }
-            if (failed) break;
-            if (!group_verbatim[g]) released[ss].store(static_cast<int64_t>(g), std::memory_order_release);
-            copied[g].store(1, std::memory_order_release);
-        }
-        if (conn) {
-            // multi-group reads: settle the deferred Completes here (their answers are long in); a single-group read (the
-            // latency path, C5) parks the connection with its last answer outstanding and the next request consumes it
-            if (NG > 1) conn->drain_pending();
-            ctx_->release(std::move(conn));
-        }
-    };
+    // ---- fetch workers.  A verbatim (framed) group's slot is only released by the verifier below, so a single fetch worker running
+    // inline on this thread would wait for itself once the groups outnumber the ring's super-slots: it gets its own thread then.
     std::vector<std::thread> threads;
-    // A verbatim (framed) group's slot is only released by the verifier below, so a single fetch worker running inline on this
-    // thread would wait for itself once the groups outnumber the ring's super-slots: it gets its own thread then.
-    if (T_threads == 1 && (NG <= NS || !any_verbatim)) worker(0, false);  // small read (FUSE-shaped, C5): no thread spawn on the latency path
+    if (P.T_threads == 1 && (P.NG <= P.NS || !P.any_verbatim)) c.worker(0, false);  // small read (FUSE-shaped, C5): no thread spawn on the latency path
     else
-        for (int t = 0; t < T_threads; t++) threads.emplace_back(worker, t, true);
+        for (int t = 0; t < P.T_threads; t++) threads.emplace_back([&c, t] { c.worker(t, true); });
 
     // ---- verifier: this thread walks the copy groups in order, `vgroups` at a time
     Err verr;
     const uint64_t launches0 = cvk_launch_count();
-    const uint64_t* d_off = reinterpret_cast<const uint64_t*>(T + o_off);
-    const uint64_t* d_len = reinterpret_cast<const uint64_t*>(T + o_len);
-    uint32_t* d_crc = reinterpret_cast<uint32_t*>(T + o_crc);
-    uint32_t* d_ferr = d_crc + J + 4;
-    CvStreamDesc* d_streams = reinterpret_cast<CvStreamDesc*>(T + o_streams);
-    CvFrameDesc* d_fdesc = reinterpret_cast<CvFrameDesc*>(T + o_fdesc);
-    for (size_t v0 = 0; v0 < NG && !verr; v0 += vgroups) {
-        const size_t v1 = std::min(NG, v0 + vgroups);
+    uint32_t* d_crc = tl.crc(T);
+    const size_t NS = P.NS;
+    for (size_t v0 = 0; v0 < P.NG && !verr; v0 += P.vgroups) {
+        const size_t v1 = std::min(P.NG, v0 + P.vgroups);
         for (size_t g = v0; g < v1; g++)
-            backoff_wait([&] { return copied[g].load(std::memory_order_acquire) != 0 || st.abort.load(); });
-        if (st.abort.load()) break;
-        const size_t g0 = v0 * k, g1 = std::min(J, v1 * k);
+            backoff_wait([&] { return c.copied[g].load(std::memory_order_acquire) != 0 || c.abort.load(); });
+        if (c.abort.load()) break;
+        const size_t g0 = v0 * P.k, g1 = std::min(J, v1 * P.k);
         uint64_t gbytes = 0;
         bool gframed = false;
         for (size_t g = v0; g < v1; g++) {
             cudaStreamWaitEvent(G.vstream, G.copy_ev[g % NS], 0);
-            gframed |= group_verbatim[g] != 0;
+            gframed |= P.group_verbatim[g] != 0;
         }
         for (size_t j = g0; j < g1; j++) gbytes += h_len[j];
         if (!gframed && bc.verify) {  // K1 over the landed bytes
-            int rc = cvk_crc_blocks(d_dst, d_off + g0, d_len + g0, static_cast<uint32_t>(g1 - g0), poly, gbytes, d_crc + g0, G.vstream);
+            int rc = cvk_crc_blocks(d_dst, tl.off(T) + g0, tl.len(T) + g0, static_cast<uint32_t>(g1 - g0), poly, gbytes, d_crc + g0, G.vstream);
             if (rc) verr = Err::io(str_printf("cvk_crc_blocks: %s", cudaGetErrorString(cudaError_t(rc))));
         }
         if (gframed) {
             // patch the request ids (known only after the fetch), expand this batch's stream descriptors, run K2
-            for (size_t j = g0; j < g1; j++) sd[j].req_id = req_ids[j];
-            cudaError_t ce = cudaMemcpyAsync(d_streams + g0, &sd[g0], sizeof(CvStreamDesc) * (g1 - g0), cudaMemcpyHostToDevice, G.vstream);
-            const uint32_t fr0 = first_frame[g0], nfr = first_frame[g1] - fr0;
+            for (size_t j = g0; j < g1; j++) sd[j].req_id = c.req_ids[j];
+            cudaError_t ce = cudaMemcpyAsync(tl.streams(T) + g0, &sd[g0], sizeof(CvStreamDesc) * (g1 - g0), cudaMemcpyHostToDevice, G.vstream);
+            const uint32_t fr0 = P.first_frame[g0], nfr = P.first_frame[g1] - fr0;
             int rc = ce != cudaSuccess ? int(ce) : 0;
-            if (!rc) rc = cvk_expand_streams(d_streams + g0, static_cast<uint32_t>(g1 - g0), d_fdesc, first_frame[J], G.vstream);
+            if (!rc) rc = cvk_expand_streams(tl.streams(T) + g0, static_cast<uint32_t>(g1 - g0), tl.fdesc(T), P.first_frame[J], G.vstream);
             if (!rc && nfr)
-                rc = cvk_unpack_frames(G.d_stage, d_fdesc + fr0, nfr, static_cast<uint32_t>(g1 - g0), d_dst, poly, gbytes,
-                                       bc.verify ? d_crc + g0 : nullptr, d_ferr + fr0, G.vstream);
+                rc = cvk_unpack_frames(G.d_stage, tl.fdesc(T) + fr0, nfr, static_cast<uint32_t>(g1 - g0), d_dst, poly, gbytes,
+                                       bc.verify ? d_crc + g0 : nullptr, tl.ferr(T) + fr0, G.vstream);
             if (rc) verr = Err::io(str_printf("cvk_unpack_frames: %s", cudaGetErrorString(cudaError_t(rc))));
             for (size_t g = v0; g < v1; g++)
-                if (group_verbatim[g]) {
+                if (P.group_verbatim[g]) {
                     cudaEventRecord(G.free_ev[g % NS], G.vstream);
-                    released[g % NS].store(static_cast<int64_t>(g), std::memory_order_release);
+                    c.released[g % NS].store(static_cast<int64_t>(g), std::memory_order_release);
                 }
         }
     }
-    if (verr) st.fail(verr);
+    if (verr) c.fail(verr);
     for (auto& th : threads) th.join();
-    if (st.err) {
+    if (c.err) {
         cudaStreamSynchronize(G.vstream);
         for (auto s : G.copy_streams) cudaStreamSynchronize(s);
-        return st.err;
+        return c.err;
     }
+
+    // ---- finish: compare the CRCs with the manifest, scatter, copy the results back, order the caller's stream after it all
     if (compare)
-        CVK_TRY(cvk_verify_crcs_masked(d_crc + f0, reinterpret_cast<const uint32_t*>(T + o_exp) + f0, T + o_skip + f0, static_cast<uint32_t>(f1 - f0), d_crc + J, nullptr,
-                                       G.vstream));
+        CVK_TRY(cvk_verify_crcs_masked(d_crc + f0, tl.expect(T) + f0, tl.skip(T) + f0, static_cast<uint32_t>(f1 - f0), d_crc + J, nullptr, G.vstream));
     if (n_segs)  // every copy group was waited for and CRC'd on vstream by now: scatter the landed bytes to their destinations
-        CVK_TRY(cvk_gather_pages(d_dst, reinterpret_cast<const CvSeg*>(T + o_segs), static_cast<uint32_t>(n_segs), pages->total, pages->d_out, G.vstream));
-    CU_TRY(cudaMemcpyAsync(G.h_result, d_crc, 4 * res_words, cudaMemcpyDeviceToHost, G.vstream));
+        CVK_TRY(cvk_gather_pages(d_dst, tl.segs(T), static_cast<uint32_t>(n_segs), pages->total, pages->d_out, G.vstream));
+    CU_TRY(cudaMemcpyAsync(G.h_result, d_crc, 4 * tl.res_words(), cudaMemcpyDeviceToHost, G.vstream));
     CU_TRY(cudaEventRecord(G.done_ev, G.vstream));
     CU_TRY(cudaStreamWaitEvent(static_cast<cudaStream_t>(user_stream), G.done_ev, 0));
-    pending_.active = true, pending_.jobs = J, pending_.frames = F;
+    pending_.active = true, pending_.jobs = J, pending_.frames = P.F;
     pending_.f0 = bc.verify ? f0 : 0, pending_.f1 = bc.verify ? f1 : 0, pending_.n_compared = compare ? n_compared : 0;
     G.pending_owner = this;
     for (size_t j = 0; j < J; j++) stats_.bytes += h_len[j];
     stats_.blocks += J;
     stats_.kernel_launches += cvk_launch_count() - launches0;
-    for (int t = 0; t < T_threads; t++) stats_.fetch_sec += fetch_sec[static_cast<size_t>(t)], stats_.h2d_bytes += h2d[static_cast<size_t>(t)];
+    for (int t = 0; t < P.T_threads; t++) stats_.fetch_sec += c.fetch_sec[static_cast<size_t>(t)], stats_.h2d_bytes += c.h2d[static_cast<size_t>(t)];
     stats_.wall_sec += now_sec() - t_start;
     stats_.reg_hits = G.reg.hits.load(), stats_.reg_misses = G.reg.misses.load();
     stats_.reg_rejected = G.reg.rejected.load(), stats_.reg_bytes = G.reg.bytes();
     stats_.ring_alloc_sec = G.ring_alloc_sec;
-    stats_.gds_bytes += gds_bytes.load();
+    stats_.gds_bytes += c.gds_bytes.load();
     return Err::ok();
 }
 

@@ -116,6 +116,9 @@ class GpuFsReader {
         std::vector<CvSeg> segs;
         uint64_t total = 0;  // sum of segs[i].len
     };
+    struct CallPlan;  // what one run_jobs call does, decided up front (plan_call)
+    struct Call;      // one run_jobs call in flight: fetch workers and the ingest paths of a copy group
+    Err plan_call(const std::vector<Job>& jobs, size_t n_segs, CallPlan* out) const;
     Err run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* stream, const Scatter* scatter = nullptr);
     Err read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const Scatter* scatter);
     FsContext* ctx_ = nullptr;
@@ -127,8 +130,8 @@ class GpuFsReader {
     uint32_t n_bad_ = 0;
     uint64_t n_bad_frames_ = 0;
     uint32_t first_frame_err_ = 0;
-    std::vector<std::shared_ptr<struct RegMapping>> held_maps_;
-    std::vector<std::shared_ptr<const FileBlocks>> held_files_;  // read_many: keeps the LocatedBlocks alive  // registered mappings with copies still in flight
+    std::vector<std::shared_ptr<struct RegMapping>> held_maps_;  // registered mappings with copies still in flight (until harvest)
+    std::vector<std::shared_ptr<const FileBlocks>> held_files_;  // read_many: keeps the LocatedBlocks alive
     struct Pending {
         bool active = false;
         size_t jobs = 0, frames = 0, f0 = 0, f1 = 0, n_compared = 0;
