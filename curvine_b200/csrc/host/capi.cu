@@ -337,32 +337,33 @@ int64_t cv_shard_plan(cv_reader* r, int32_t rank, int32_t world, int64_t* block_
     API_GUARD_END
 }
 
+// a plain range is a strided range of one row
 static std::vector<ReadvRange> readv_ranges(const CvRange* ranges, int32_t n) {
     std::vector<ReadvRange> out;
     for (int32_t i = 0; ranges && i < n; i++) out.push_back(ReadvRange{ranges[i].file_off, ranges[i].len, static_cast<uint8_t*>(ranges[i].d_dst)});
     return out;
 }
 
-int64_t cv_readv_device(cv_reader* r, const CvRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes) {
-    API_GUARD_BEGIN
-    API_NEED(r);
-    API_NEED(nbytes);
-    if (n > 0) API_NEED(ranges);
+static std::vector<ReadvRange> strided_ranges(const CvStridedRange* ranges, int32_t n) {
+    std::vector<ReadvRange> out;
+    for (int32_t i = 0; ranges && i < n; i++) {
+        const CvStridedRange& s = ranges[i];
+        out.push_back(ReadvRange{s.file_off, s.row_len, static_cast<uint8_t*>(s.d_dst), s.rows, s.file_pitch, s.dst_pitch});
+    }
+    return out;
+}
+
+static int64_t readv_device_common(cv_reader* r, const std::vector<ReadvRange>& rs, int32_t n, cv_stream_t stream, int64_t* nbytes) {
     API_TRY(ensure_dev(r));
-    const std::vector<ReadvRange> rs = readv_ranges(ranges, n);
     int64_t got = 0;
     API_TRY(r->dev->readv_device(rs.data(), n, stream, &got));
     *nbytes = got;
     return ok();
-    API_GUARD_END
 }
 
-int64_t cv_readv_plan(cv_reader* r, const CvRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len, int32_t* range_index,
-                      int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes) {
-    API_GUARD_BEGIN
-    API_NEED(r);
-    if (n > 0) API_NEED(ranges);
-    const std::vector<ReadvRange> rs = readv_ranges(ranges, n);
+// The plan's spans into the caller's arrays (any of which may be NULL); `rows` only for the strided form.
+static int64_t readv_plan_common(cv_reader* r, const std::vector<ReadvRange>& rs, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len,
+                                 int64_t* rows, int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes) {
     const FileBlocks& fb = r->host->file_blocks();
     std::vector<ReadvBlock> blocks;
     std::vector<ReadvSpan> spans;
@@ -376,6 +377,7 @@ int64_t cv_readv_plan(cv_reader* r, const CvRange* ranges, int32_t n, int64_t* b
             if (block_index) block_index[i] = static_cast<int64_t>(b.block);
             if (block_off) block_off[i] = spans[k].block_off;
             if (len) len[i] = spans[k].len;
+            if (rows) rows[i] = spans[k].rows;
             if (range_index) range_index[i] = spans[k].range;
             if (direct) direct[i] = b.direct ? 1 : 0;
         }
@@ -384,6 +386,42 @@ int64_t cv_readv_plan(cv_reader* r, const CvRange* ranges, int32_t n, int64_t* b
     if (n_blocks) *n_blocks = static_cast<int64_t>(blocks.size());
     if (fetch_bytes) *fetch_bytes = fetched;
     return ok();
+}
+
+int64_t cv_readv_device(cv_reader* r, const CvRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes) {
+    API_GUARD_BEGIN
+    API_NEED(r);
+    API_NEED(nbytes);
+    if (n > 0) API_NEED(ranges);
+    return readv_device_common(r, readv_ranges(ranges, n), n, stream, nbytes);
+    API_GUARD_END
+}
+
+int64_t cv_readv_plan(cv_reader* r, const CvRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len, int32_t* range_index,
+                      int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes) {
+    API_GUARD_BEGIN
+    API_NEED(r);
+    if (n > 0) API_NEED(ranges);
+    return readv_plan_common(r, readv_ranges(ranges, n), n, block_index, block_off, len, nullptr, range_index, direct, cap, n_spans, n_blocks,
+                             fetch_bytes);
+    API_GUARD_END
+}
+
+int64_t cv_readv_strided_device(cv_reader* r, const CvStridedRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes) {
+    API_GUARD_BEGIN
+    API_NEED(r);
+    API_NEED(nbytes);
+    if (n > 0) API_NEED(ranges);
+    return readv_device_common(r, strided_ranges(ranges, n), n, stream, nbytes);
+    API_GUARD_END
+}
+
+int64_t cv_readv_strided_plan(cv_reader* r, const CvStridedRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len, int64_t* rows,
+                              int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes) {
+    API_GUARD_BEGIN
+    API_NEED(r);
+    if (n > 0) API_NEED(ranges);
+    return readv_plan_common(r, strided_ranges(ranges, n), n, block_index, block_off, len, rows, range_index, direct, cap, n_spans, n_blocks, fetch_bytes);
     API_GUARD_END
 }
 
@@ -857,6 +895,13 @@ int64_t cv_synth_create_file(cv_worker* w, const char* path, int64_t inode_id, i
     }
     return ok();
     API_GUARD_END
+}
+
+// The host sources are also linked without csrc/kernels.cu (the host-only test library of tests/mock_cuda, whose CPU stand-ins cover the
+// launchers that existed before this one).  There this weak definition keeps the symbol resolvable and reports the strided gather as
+// unsupported; it copies nothing.  Every library that links kernels.cu gets the kernel: the strong definition there replaces this one.
+__attribute__((weak)) int cvk_gather_strided(const uint8_t*, const CvStridedSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) {
+    return n ? int(cudaErrorNotSupported) : 0;
 }
 
 }  // extern "C"

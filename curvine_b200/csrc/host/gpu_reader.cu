@@ -357,32 +357,70 @@ Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::v
     if (n > 0 && !ranges) return Err::common("readv: null range table");
     const int64_t flen = fb.status.len;
     std::vector<int32_t> order;
+    std::vector<int64_t> extent(static_cast<size_t>(n));  // file bytes from row 0's first byte to the last row's last byte
     for (int32_t i = 0; i < n; i++) {
         const ReadvRange& r = ranges[i];
-        if (r.len < 0) return Err::common(str_printf("readv: range %d has a negative length (%lld)", i, (long long)r.len));
-        if (r.file_off < 0 || r.file_off > flen || r.len > flen - r.file_off)
-            return Err::common(str_printf("readv: range %d [%lld, +%lld) lies outside the file (%lld bytes)", i, (long long)r.file_off, (long long)r.len, (long long)flen));
-        if (r.len > 0) order.push_back(i);
+        if (r.row_len < 0) return Err::common(str_printf("readv: range %d has a negative length (%lld)", i, (long long)r.row_len));
+        if (r.rows < 0) return Err::common(str_printf("readv: range %d has a negative row count (%lld)", i, (long long)r.rows));
+        if (r.file_pitch < 0 || r.dst_pitch < 0) return Err::common(str_printf("readv: range %d has a negative pitch", i));
+        if (r.rows > 1 && (r.file_pitch < r.row_len || r.dst_pitch < r.row_len))
+            return Err::common(str_printf("readv: range %d has a pitch shorter than its row length (%lld)", i, (long long)r.row_len));
+        int64_t& ext = extent[static_cast<size_t>(i)];
+        ext = r.rows == 0 ? 0 : r.row_len;
+        for (int64_t pitch : {r.file_pitch, r.dst_pitch})
+            if (r.rows > 1 && pitch > 0 && r.rows - 1 > (INT64_MAX - r.row_len) / pitch)
+                return Err::common(str_printf("readv: range %d: (rows - 1) * pitch + row_len overflows", i));
+        if (r.rows > 1) ext += (r.rows - 1) * r.file_pitch;
+        if (r.file_off < 0 || r.file_off > flen || ext > flen - r.file_off)
+            return Err::common(str_printf("readv: range %d [%lld, +%lld) lies outside the file (%lld bytes)", i, (long long)r.file_off, (long long)ext, (long long)flen));
+        if (r.row_len > 0 && r.rows > 0) order.push_back(i);
     }
     std::sort(order.begin(), order.end(), [&](int32_t a, int32_t b) { return ranges[a].file_off < ranges[b].file_off; });
     for (size_t k = 1; k < order.size(); k++)
-        if (ranges[order[k]].file_off < ranges[order[k - 1]].file_off + ranges[order[k - 1]].len)
+        if (ranges[order[k]].file_off < ranges[order[k - 1]].file_off + extent[static_cast<size_t>(order[k - 1])])
             return Err::common(str_printf("readv: ranges %d and %d overlap in the file", order[k - 1], order[k]));
     for (int32_t i : order) {
-        for (int64_t p = ranges[i].file_off, end = p + ranges[i].len; p < end;) {
+        const ReadvRange& r = ranges[i];
+        const int64_t L = r.row_len, R = r.rows, P = R > 1 ? r.file_pitch : L, off = r.file_off;
+        // next byte to place: column `col` of row `row`.  Every pass of the loop handles one touched block, in file order.
+        int64_t row = 0, col = 0;
+        while (row < R) {
+            const int64_t q = off + row * P + col;
             int64_t boff;
             size_t idx;
-            CV_RETURN_IF_ERR(fb.get_read_block(p, &boff, &idx));
-            const int64_t take = std::min(end - p, fb.block_locs[idx].block.len - boff);
+            CV_RETURN_IF_ERR(fb.get_read_block(q, &boff, &idx));
+            const int64_t bs = q - boff, be = bs + fb.block_locs[idx].block.len;
             if (blocks->empty() || blocks->back().block != idx) blocks->push_back(ReadvBlock{idx, false, spans->size(), 0});
-            spans->push_back(ReadvSpan{boff, take, i});
-            blocks->back().n_spans++;
-            p += take;
+            auto emit = [&](int64_t at, int64_t len, int64_t rows, int64_t dst_off) {
+                spans->push_back(ReadvSpan{at - bs, len, rows, dst_off, i});
+                blocks->back().n_spans++;
+            };
+            // the row in progress, when it began in an earlier block or runs past this one: clipped by the block's edge
+            if (col > 0 || off + row * P + L > be) {
+                const int64_t take = std::min(L - col, be - q);
+                emit(q, take, 1, row * r.dst_pitch + col);
+                col += take;
+                if (col < L) continue;  // it goes on in the next block
+                row++, col = 0;
+            }
+            // the whole rows that start and end inside the block
+            if (row < R && off + row * P + L <= be) {
+                const int64_t last = std::min(R - 1, (be - L - off) / P);
+                emit(off + row * P, L, last - row + 1, row * r.dst_pitch);
+                row = last + 1;
+            }
+            // a row that starts inside the block and runs past its end
+            if (row < R && off + row * P < be) {
+                const int64_t take = be - (off + row * P);
+                emit(off + row * P, take, 1, row * r.dst_pitch);
+                col = take;
+            }
+            // otherwise the next row starts in a later block: the next pass looks that block up directly
         }
     }
     for (ReadvBlock& b : *blocks) {
         const ReadvSpan& s = (*spans)[b.first_span];
-        b.direct = b.n_spans == 1 && s.block_off == 0 && s.len == fb.block_locs[b.block].block.len;
+        b.direct = b.n_spans == 1 && s.rows == 1 && s.block_off == 0 && s.len == fb.block_locs[b.block].block.len;
     }
     return Err::ok();
 }
@@ -554,16 +592,17 @@ static Err check_device_dst(const void* p, int device) {
 enum JobMode : uint8_t { kPlain = 0, kFramed = 1, kHole = 3 };
 
 // Layout of the per-call device tables (shared by all readers of the context) and of their pinned host image:
-//   off[J] len[J] expect[J] skip[J] | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F] | segs[n_segs]
+//   off[J] len[J] expect[J] skip[J] | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F] | segs[n_segs] | strided[n_strided]
 // off .. skip are uploaded before the fetch starts; crc .. ferr are the results copied back.
 struct TableLayout {
-    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, o_segs = 0, bytes = 0;
+    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, o_segs = 0, o_strided = 0, bytes = 0;
     TableLayout() = default;
-    TableLayout(size_t j, size_t f, size_t n_segs) : J(j), F(f) {
+    TableLayout(size_t j, size_t f, size_t n_segs, size_t n_strided) : J(j), F(f) {
         auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
         o_len = up(8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_crc = up(o_skip + J);
         o_streams = up(o_crc + 4 * res_words()), o_fdesc = up(o_streams + sizeof(CvStreamDesc) * J);
-        o_segs = up(o_fdesc + sizeof(CvFrameDesc) * F), bytes = up(o_segs + sizeof(CvSeg) * n_segs);
+        o_segs = up(o_fdesc + sizeof(CvFrameDesc) * F), o_strided = up(o_segs + sizeof(CvSeg) * n_segs);
+        bytes = up(o_strided + sizeof(CvStridedSeg) * n_strided);
     }
     size_t res_words() const { return J + 4 + F; }
     uint64_t* off(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t); }
@@ -575,6 +614,7 @@ struct TableLayout {
     CvStreamDesc* streams(uint8_t* t) const { return reinterpret_cast<CvStreamDesc*>(t + o_streams); }
     CvFrameDesc* fdesc(uint8_t* t) const { return reinterpret_cast<CvFrameDesc*>(t + o_fdesc); }
     CvSeg* segs(uint8_t* t) const { return reinterpret_cast<CvSeg*>(t + o_segs); }
+    CvStridedSeg* strided(uint8_t* t) const { return reinterpret_cast<CvStridedSeg*>(t + o_strided); }
 };
 
 // What one run_jobs call does, decided before any CUDA call.
@@ -594,7 +634,7 @@ struct GpuFsReader::CallPlan {
     TableLayout tl;
 };
 
-Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, CallPlan* out) const {
+Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, CallPlan* out) const {
     CallPlan& P = *out;
     const B200Conf& bc = ctx_->conf.b200;
     const size_t J = jobs.size();
@@ -640,7 +680,7 @@ Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, CallPlan
     P.group_verbatim.assign(P.NG, 0);
     for (size_t j = 0; j < J; j++) P.group_verbatim[j / P.k] |= P.mode[j] == kFramed;
     P.T_threads = static_cast<int>(std::min<size_t>(static_cast<size_t>(std::max(1, bc.fetch_threads)), P.NG));
-    P.tl = TableLayout(J, P.F, n_segs);
+    P.tl = TableLayout(J, P.F, n_segs, n_strided);
     return Err::ok();
 }
 
@@ -992,10 +1032,10 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     CU_TRY(cudaStreamWaitEvent(G.vstream, G.entry_ev, 0));
     const B200Conf& bc = ctx_->conf.b200;
     const int poly = bc.verify_poly ? 1 : 0;
-    const size_t n_segs = pages ? pages->segs.size() : 0;
+    const size_t n_segs = pages ? pages->segs.size() : 0, n_strided = pages ? pages->strided.size() : 0;
 
     CallPlan P;
-    CV_RETURN_IF_ERR(plan_call(jobs, n_segs, &P));
+    CV_RETURN_IF_ERR(plan_call(jobs, n_segs, n_strided, &P));
     Call c(*this, jobs, P, d_dst);
     if (!(bc.zero_copy && !P.call_framed)) CV_RETURN_IF_ERR(c.ensure_ring());
 
@@ -1026,6 +1066,10 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     if (n_segs) {  // the scatter's segment table rides in the same pinned image
         memcpy(tl.segs(h), pages->segs.data(), sizeof(CvSeg) * n_segs);
         CU_TRY(cudaMemcpyAsync(tl.segs(T), tl.segs(h), sizeof(CvSeg) * n_segs, cudaMemcpyHostToDevice, G.vstream));
+    }
+    if (n_strided) {  // and so does its table of strided segments
+        memcpy(tl.strided(h), pages->strided.data(), sizeof(CvStridedSeg) * n_strided);
+        CU_TRY(cudaMemcpyAsync(tl.strided(T), tl.strided(h), sizeof(CvStridedSeg) * n_strided, cudaMemcpyHostToDevice, G.vstream));
     }
     CU_TRY(cudaMemsetAsync(tl.crc(T), 0, 4 * tl.res_words(), G.vstream));
     CvStreamDesc* sd = tl.streams(h);
@@ -1102,6 +1146,8 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
         CVK_TRY(cvk_verify_crcs_masked(d_crc + f0, tl.expect(T) + f0, tl.skip(T) + f0, static_cast<uint32_t>(f1 - f0), d_crc + J, nullptr, G.vstream));
     if (n_segs)  // every copy group was waited for and CRC'd on vstream by now: scatter the landed bytes to their destinations
         CVK_TRY(cvk_gather_pages(d_dst, tl.segs(T), static_cast<uint32_t>(n_segs), pages->total, pages->d_out, G.vstream));
+    if (n_strided)  // spans of several rows each
+        CVK_TRY(cvk_gather_strided(d_dst, tl.strided(T), static_cast<uint32_t>(n_strided), pages->strided_total, pages->d_out, G.vstream));
     CU_TRY(cudaMemcpyAsync(G.h_result, d_crc, 4 * tl.res_words(), cudaMemcpyDeviceToHost, G.vstream));
     CU_TRY(cudaEventRecord(G.done_ev, G.vstream));
     CU_TRY(cudaStreamWaitEvent(static_cast<cudaStream_t>(user_stream), G.done_ev, 0));
@@ -1160,11 +1206,12 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
     int64_t total = 0;
     uintptr_t lo = UINTPTR_MAX;
     for (int32_t i = 0; i < n_ranges; i++) {
-        if (ranges[i].len == 0) continue;
-        CV_RETURN_IF_ERR(check_device_dst(ranges[i].dst, G.device).ctx(str_printf("range %d", i)));
-        CV_RETURN_IF_ERR(check_device_dst(ranges[i].dst + ranges[i].len - 1, G.device).ctx(str_printf("range %d (last byte)", i)));
-        lo = std::min(lo, reinterpret_cast<uintptr_t>(ranges[i].dst));
-        total += ranges[i].len;
+        const ReadvRange& r = ranges[i];
+        if (r.row_len == 0 || r.rows == 0) continue;
+        CV_RETURN_IF_ERR(check_device_dst(r.dst, G.device).ctx(str_printf("range %d", i)));
+        CV_RETURN_IF_ERR(check_device_dst(r.dst + (r.rows - 1) * r.dst_pitch + r.row_len - 1, G.device).ctx(str_printf("range %d (last byte)", i)));
+        lo = std::min(lo, reinterpret_cast<uintptr_t>(r.dst));
+        total += r.rows * r.row_len;
     }
     if (blocks.empty()) return Err::ok();
     std::vector<size_t> boundary;
@@ -1185,10 +1232,10 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
     // every destination is addressed relative to the lowest one (or the staging): one base pointer, unsigned offsets
     uint8_t* base = reinterpret_cast<uint8_t*>(lo);
     auto rel = [lo](const uint8_t* p) { return static_cast<int64_t>(reinterpret_cast<uintptr_t>(p) - lo); };
-    auto dst_of = [&](const ReadvBlock& b, const ReadvSpan& s) { return rel(ranges[s.range].dst) + fb.starts[b.block] + s.block_off - ranges[s.range].file_off; };
+    auto dst_of = [&](const ReadvSpan& s) { return rel(ranges[s.range].dst) + s.dst_off; };
     std::vector<Job> jobs;
     for (const ReadvBlock& b : blocks)
-        if (b.direct) jobs.push_back(Job{&fb.block_locs[b.block], 0, spans[b.first_span].len, dst_of(b, spans[b.first_span]), true});
+        if (b.direct) jobs.push_back(Job{&fb.block_locs[b.block], 0, spans[b.first_span].len, dst_of(spans[b.first_span]), true});
     size_t next = 0;
     do {
         Scatter sc;
@@ -1198,11 +1245,19 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
             const int64_t at = rel(stage + slot * static_cast<size_t>(stage_block));
             jobs.push_back(Job{&fb.block_locs[b.block], 0, fb.block_locs[b.block].block.len, at, true});
             for (size_t k = b.first_span; k < b.first_span + b.n_spans; k++) {
-                sc.segs.push_back(CvSeg{static_cast<uint64_t>(at + spans[k].block_off), static_cast<uint64_t>(dst_of(b, spans[k])), static_cast<uint64_t>(spans[k].len)});
-                sc.total += static_cast<uint64_t>(spans[k].len);
+                const ReadvSpan& s = spans[k];
+                const uint64_t src = static_cast<uint64_t>(at + s.block_off), dst = static_cast<uint64_t>(dst_of(s)), len = static_cast<uint64_t>(s.len);
+                if (s.rows == 1) {
+                    sc.segs.push_back(CvSeg{src, dst, len});
+                    sc.total += len;
+                } else {
+                    const ReadvRange& r = ranges[s.range];
+                    sc.strided.push_back(CvStridedSeg{src, dst, len, static_cast<uint64_t>(s.rows), static_cast<uint64_t>(r.file_pitch), static_cast<uint64_t>(r.dst_pitch)});
+                    sc.strided_total += len * static_cast<uint64_t>(s.rows);
+                }
             }
         }
-        CV_RETURN_IF_ERR(run_jobs(jobs, base, stream, sc.segs.empty() ? nullptr : &sc));
+        CV_RETURN_IF_ERR(run_jobs(jobs, base, stream, sc.segs.empty() && sc.strided.empty() ? nullptr : &sc));
         jobs.clear();
     } while (next < boundary.size());
     *n = total;

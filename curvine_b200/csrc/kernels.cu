@@ -143,6 +143,25 @@ __global__ void prep_segs_kernel(const uint8_t* src, const CvSeg* segs, uint32_t
     counts[i] = piece_geom<true>(p, seg_shift).units;
 }
 
+// K3 over 2D descriptors, one train: rows [base, base + cnt) of the row numbering row_pref gives (descriptor d owns rows
+// [row_pref[d], row_pref[d + 1])).  One warp per descriptor, lanes stride over its rows inside the train, one piece per row.
+__global__ void prep_strided_kernel(const uint8_t* src, const CvStridedSeg* segs, const uint64_t* row_pref, uint32_t n, uint8_t* dst,
+                                    uint64_t base, uint32_t cnt, uint32_t seg_shift, Piece* pieces, uint32_t* counts) {
+    const uint32_t d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (d >= n) return;
+    const uint64_t r0 = row_pref[d], r1 = row_pref[d + 1];
+    const uint64_t lo = r0 > base ? r0 : base, hi = r1 < base + cnt ? r1 : base + cnt;
+    if (lo >= hi) return;
+    const CvStridedSeg s = segs[d];
+    for (uint64_t g = lo + lane; g < hi; g += 32) {
+        const uint64_t k = g - r0;
+        Piece p{src + s.src_off + k * s.src_pitch, dst + s.dst_off + k * s.dst_pitch, s.len};
+        pieces[g - base] = p;
+        counts[g - base] = piece_geom<true>(p, seg_shift).units;
+    }
+}
+
 __global__ void prep_deinterleave_kernel(const uint8_t* gathered, uint64_t shard_stride, uint32_t world,
                                          uint64_t block_size, uint64_t n_blocks, uint64_t file_len, uint8_t* dst,
                                          uint32_t seg_shift, Piece* pieces, uint32_t* counts) {
@@ -993,6 +1012,8 @@ static int ensure_device(int* dev_out) {
 
 static std::atomic<bool> g_small_path{true};  // cvk_tune(5, 0/1): single-launch kernels for inputs of at most ~1 MiB
 static std::atomic<int> g_seg_shift_override{0};  // cvk_tune(4, s): segment size 2^s for every launcher (0 = chosen from the input size)
+constexpr uint32_t kStridedTrainRows = 1u << 22;
+static std::atomic<uint32_t> g_strided_train{kStridedTrainRows};  // cvk_tune(6, r): rows per train of cvk_gather_strided
 static uint32_t pick_seg_shift(uint64_t total_bytes, int sm_count) {
     if (const int o = g_seg_shift_override.load(std::memory_order_relaxed)) return static_cast<uint32_t>(o);
     // ~16 units per warp keeps the contiguous per-CTA ranges balanced for big inputs; small inputs get 16 KiB segments
@@ -1133,6 +1154,7 @@ int cvk_tune(int what, int value) {
     else if (what == 3 && (value == 0 || value == 1)) g_staged.store(value != 0);
     else if (what == 4 && (value == 0 || (value >= 12 && value <= 20))) g_seg_shift_override.store(value);
     else if (what == 5 && (value == 0 || value == 1)) g_small_path.store(value != 0);
+    else if (what == 6 && value >= 0 && value <= int(kStridedTrainRows)) g_strided_train.store(value ? uint32_t(value) : kStridedTrainRows);
     else return int(cudaErrorInvalidValue);
     return 0;
 }
@@ -1199,12 +1221,7 @@ int cvk_crc_blocks(const uint8_t* d_base, const uint64_t* d_off, const uint64_t*
 
 int cvk_verify_crcs(const uint32_t* d_crc, const uint32_t* d_expect, uint32_t n, uint32_t* d_n_bad,
                     uint8_t* d_bad_mask, cv_stream_t stream) {
-    if (n == 0) return 0;
-    DeviceGuard guard(d_crc);
-    verify_crcs_kernel<<<cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(d_crc, d_expect, nullptr, n, d_n_bad,
-                                                                                   d_bad_mask);
-    count_launch();
-    return int(cudaGetLastError());
+    return cvk_verify_crcs_masked(d_crc, d_expect, nullptr, n, d_n_bad, d_bad_mask, stream);
 }
 
 int cvk_verify_crcs_masked(const uint32_t* d_crc, const uint32_t* d_expect, const uint8_t* d_skip, uint32_t n, uint32_t* d_n_bad,
@@ -1305,6 +1322,41 @@ int cvk_gather_pages(const uint8_t* d_src, const CvSeg* d_segs, uint32_t n, uint
     prep_segs_kernel<<<cdiv(n, 256), 256, 0, st>>>(d_src, d_segs, n, d_dst, seg_shift, w.pieces, w.counts);
     count_launch();
     return copy_pieces(w, n, seg_shift, dev, st);
+}
+
+int cvk_gather_strided(const uint8_t* d_src, const CvStridedSeg* d_segs, uint32_t n, uint64_t total_bytes, uint8_t* d_dst,
+                       cv_stream_t stream) {
+    if (n == 0) return 0;
+    DeviceGuard guard(d_dst);
+    int dev;
+    if (int rc = ensure_device(&dev)) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // the row numbering: descriptor d owns rows [pref[d], pref[d + 1]); a descriptor of empty rows owns none
+    std::vector<CvStridedSeg> h(n);
+    CV_TRY(cudaMemcpyAsync(h.data(), d_segs, sizeof(CvStridedSeg) * n, cudaMemcpyDeviceToHost, st));
+    CV_TRY(cudaStreamSynchronize(st));
+    std::vector<uint64_t> pref(size_t(n) + 1, 0);
+    for (uint32_t d = 0; d < n; d++) pref[d + 1] = pref[d] + (h[d].len ? h[d].rows : 0);
+    const uint64_t rows = pref[n];
+    if (rows == 0) return 0;
+    uint64_t* d_pref = nullptr;
+    CV_TRY(cudaMallocFromPoolAsync(reinterpret_cast<void**>(&d_pref), sizeof(uint64_t) * pref.size(), g_pool[dev], st));
+    cudaError_t ce = cudaMemcpyAsync(d_pref, pref.data(), sizeof(uint64_t) * pref.size(), cudaMemcpyHostToDevice, st);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);  // pref is this frame's (pageable) vector
+    int rc = int(ce);
+    const uint32_t seg_shift = pick_seg_shift(total_bytes, g_sm_count[dev]);
+    const uint64_t train = g_strided_train.load(std::memory_order_relaxed);
+    // one launch train per `train` rows: the workspace is bounded by the train, not by the row count
+    for (uint64_t base = 0; base < rows && !rc; base += train) {
+        const uint32_t cnt = uint32_t(rows - base < train ? rows - base : train);
+        Workspace w;
+        if ((rc = ws_alloc(&w, dev, cnt, 0, total_bytes, seg_shift, st))) break;
+        prep_strided_kernel<<<cdiv(uint64_t(n) * 32, 256), 256, 0, st>>>(d_src, d_segs, d_pref, n, d_dst, base, cnt, seg_shift, w.pieces, w.counts);
+        count_launch();
+        rc = copy_pieces(w, cnt, seg_shift, dev, st);
+    }
+    const cudaError_t freed = cudaFreeAsync(d_pref, st);
+    return rc ? rc : int(freed);
 }
 
 int cvk_deinterleave_blocks(const uint8_t* d_gathered, uint64_t shard_stride, uint32_t world, uint64_t block_size,

@@ -166,11 +166,12 @@ class CurvineClient:
         finally:
             reader.close()
 
-    def load_safetensors(self, path, device=None, names=None):
-        """Addition: a safetensors checkpoint as {name: CUDA tensor}, from one CRC-verified vectored read (curvine_b200.safetensors)."""
+    def load_safetensors(self, path, device=None, names=None, slices=None):
+        """Addition: a safetensors checkpoint as {name: CUDA tensor}, from one CRC-verified vectored read (curvine_b200.safetensors);
+        slices = {name: (dim, start, stop)} loads only that part of a tensor (a tensor-parallel rank's shard)."""
         from . import safetensors
         try:
-            return safetensors.load_file(self.file_system_ptr, path, device=device, names=names)
+            return safetensors.load_file(self.file_system_ptr, path, device=device, names=names, slices=slices)
         except _fs.FsError as e:
             raise IOError("Native load safetensors failed: %s" % e)
 

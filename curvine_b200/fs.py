@@ -203,6 +203,39 @@ class Reader:
         spans = [(a64[0][i], a64[1][i], a64[2][i], a32[0][i], bool(a32[1][i])) for i in range(ns.value)]
         return spans, nb.value, fb.value
 
+    @staticmethod
+    def _strided_ranges(ranges):
+        arr = (_lib.CvStridedRange * max(1, len(ranges)))()
+        for i, (off, row_len, rows, file_pitch, ptr, dst_pitch) in enumerate(ranges):
+            a = arr[i]
+            a.file_off, a.row_len, a.rows, a.file_pitch, a.d_dst, a.dst_pitch = off, row_len, rows, file_pitch, ptr, dst_pitch
+        return arr
+
+    def readv_strided_device(self, ranges, stream: int = 0) -> int:
+        """Strided device read: `ranges` is a list of (file_off, row_len, rows, file_pitch, d_ptr, dst_pitch); row k of a range is file
+        bytes [file_off + k*file_pitch, +row_len) and lands at d_ptr + k*dst_pitch.  Verified and ordered like readv_device.
+        -> sum of rows * row_len."""
+        n = ctypes.c_int64()
+        _check(_lib.lib().cv_readv_strided_device(self._h, self._strided_ranges(ranges), len(ranges), ctypes.c_void_p(stream), ctypes.byref(n)))
+        return n.value
+
+    def readv_strided_plan(self, ranges):
+        """What readv_strided_device(ranges) executes (host-only; d_ptr is not looked at).  -> (spans, n_blocks, fetch_bytes) with spans in
+        file order as (block_index, block_off, len, rows, range_index, direct): rows k < rows of the span are bytes
+        [block_off + k*file_pitch, +len) of the block."""
+        arr = self._strided_ranges(ranges)
+        ns, nb, fb = ctypes.c_int32(), ctypes.c_int64(), ctypes.c_int64()
+        L = _lib.lib()
+        _check(L.cv_readv_strided_plan(self._h, arr, len(ranges), None, None, None, None, None, None, 0, ctypes.byref(ns), ctypes.byref(nb),
+                                       ctypes.byref(fb)))
+        cap = max(1, ns.value)
+        a64 = [(ctypes.c_int64 * cap)() for _ in range(4)]
+        a32 = [(ctypes.c_int32 * cap)() for _ in range(2)]
+        _check(L.cv_readv_strided_plan(self._h, arr, len(ranges), a64[0], a64[1], a64[2], a64[3], a32[0], a32[1], cap, ctypes.byref(ns),
+                                       ctypes.byref(nb), ctypes.byref(fb)))
+        spans = [(a64[0][i], a64[1][i], a64[2][i], a64[3][i], a32[0][i], bool(a32[1][i])) for i in range(ns.value)]
+        return spans, nb.value, fb.value
+
     def fuse_read_device(self, pos: int, size: int, d_scratch: int, d_page_base: int, page_offsets, page_size: int,
                          stream: int = 0) -> int:
         arr = (ctypes.c_uint64 * len(page_offsets))(*page_offsets)

@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import CvFrameDesc, CvSeg, CvStreamDesc, check
+from ._lib import CvFrameDesc, CvSeg, CvStreamDesc, CvStridedSeg, check
 
 POLY_IEEE, POLY_CASTAGNOLI = 0, 1
 
@@ -96,6 +96,17 @@ def pack_frames(src, d_desc, n_frames, n_blocks, wire, poly, total_bytes, want_c
 def gather_pages(src, d_segs, n, total_bytes, dst, stream=None):
     check(_lib.lib().cvk_gather_pages(_ptr(src), _ptr(d_segs), n, total_bytes, _ptr(dst), _stream_ptr(stream)),
           "cvk_gather_pages")
+
+
+def strided_segs_to_device(segs, device):
+    """segs: list of (src_off, dst_off, len, rows, src_pitch, dst_pitch)"""
+    arr = (CvStridedSeg * len(segs))(*[CvStridedSeg(*s) for s in segs])
+    return _struct_array_to_device(arr, device)
+
+
+def gather_strided(src, d_segs, n, total_bytes, dst, stream=None):
+    check(_lib.lib().cvk_gather_strided(_ptr(src), _ptr(d_segs), n, total_bytes, _ptr(dst), _stream_ptr(stream)),
+          "cvk_gather_strided")
 
 
 def deinterleave_blocks(gathered, shard_stride, world, block_size, n_blocks, file_len, dst, stream=None):

@@ -5,8 +5,9 @@ The format needs no dependency: an 8-byte little-endian header length, a JSON ob
 {"dtype", "shape", "data_offsets": [begin, end]} (offsets relative to the first byte after the header), an optional "__metadata__"
 entry, then the raw little-endian tensor bytes."""
 import json
+import numbers
 import struct
-from typing import Callable, Dict, Iterable, Optional, Tuple
+from typing import Callable, Dict, Iterable, List, Optional, Tuple
 
 from . import fs as _fs
 
@@ -81,36 +82,108 @@ def parse_header(read: Callable[[int, int], bytes], file_len: int) -> Tuple[int,
     return data_start, out
 
 
+def _open_header(fs, path):
+    """-> (reader, data_start, entries) of safetensors file `path`; the caller completes the reader."""
+    r = fs.open(path)
+
+    def read(off, n):
+        r.seek(off)
+        b = r.read_full(n)
+        if len(b) != n:
+            raise SafetensorsError("short read of the header: %d of %d bytes" % (len(b), n))
+        return b
+
+    try:
+        data_start, entries = parse_header(read, r.len())
+    except BaseException:
+        r.complete()
+        raise
+    return r, data_start, entries
+
+
+def read_header(fs: "_fs.CurvineFileSystem", path: str) -> Dict[str, tuple]:
+    """{name: (torch dtype, shape)} of safetensors file `path`, from its header alone: what a tensor-parallel rank needs to compute the
+    `slices` it passes to load_file."""
+    r, _, entries = _open_header(fs, path)
+    r.complete()
+    return {name: (dt, shape) for name, (dt, shape, _, _) in entries.items()}
+
+
+def _is_integral(x) -> bool:
+    return isinstance(x, numbers.Integral) and not isinstance(x, bool)
+
+
+def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=None) -> List[tuple]:
+    """The loader's ranges, without a GPU.  -> [(name, dtype, shape of the result, range)] for the selected names, in order, where range
+    is (file_off, row_len, rows, file_pitch, dst_pitch) of Reader.readv_strided_device (d_ptr left out), or None when the tensor has no
+    bytes to read.  An unsliced tensor is one row.  slices[name] = (dim, start, stop) keeps [start, stop) of dimension dim: the rows are
+    the prod(shape[:dim]) pieces of the row-major tensor that hold it, each (stop - start) * inner bytes long and shape[dim] * inner bytes
+    apart (inner = prod(shape[dim+1:]) * itemsize), landing back to back.  Raises KeyError for a sliced name the file does not hold,
+    ValueError for a malformed slice or a sliced name outside `selected`."""
+    slices = dict(slices or {})
+    sel = set(selected)
+    for name, spec in slices.items():
+        if name not in entries:
+            raise KeyError("the file holds no tensor named %r" % (name,))
+        if name not in sel:
+            raise ValueError("%s is sliced but not among the selected names" % name)
+        if not isinstance(spec, (tuple, list)) or len(spec) != 3 or not all(_is_integral(x) for x in spec):
+            raise ValueError("%s: slice %r is not (dim, start, stop) of integers" % (name, spec))
+        shape = entries[name][1]
+        dim, start, stop = (int(x) for x in spec)
+        if not shape:
+            raise ValueError("%s: a 0-d tensor cannot be sliced" % name)
+        if not -len(shape) <= dim < len(shape):
+            raise ValueError("%s: dim %d is out of range for a %d-d tensor" % (name, dim, len(shape)))
+        d = dim % len(shape)
+        if not 0 <= start <= stop <= shape[d]:
+            raise ValueError("%s: [%d, %d) is not a slice of dimension %d of size %d" % (name, start, stop, dim, shape[d]))
+    out = []
+    for name in selected:
+        dtype, shape, begin, end = entries[name]
+        if name not in slices:
+            out.append((name, dtype, shape, (data_start + begin, end - begin, 1, 0, 0) if end > begin else None))
+            continue
+        dim, start, stop = (int(x) for x in slices[name])
+        d = dim % len(shape)
+        inner = dtype.itemsize
+        for x in shape[d + 1:]:
+            inner *= x
+        rows = 1
+        for x in shape[:d]:
+            rows *= x
+        row_len = (stop - start) * inner
+        res = shape[:d] + (stop - start,) + shape[d + 1:]
+        rng = (data_start + begin + start * inner, row_len, rows, shape[d] * inner, row_len) if row_len and rows else None
+        out.append((name, dtype, res, rng))
+    return out
+
+
 def load_file(fs: "_fs.CurvineFileSystem", path: str, device=None, names: Optional[Iterable[str]] = None,
-              verify: bool = True) -> Dict[str, "object"]:
+              verify: bool = True, slices: Optional[Dict[str, tuple]] = None) -> Dict[str, "object"]:
     """The tensors of safetensors file `path` (all of them, or those in `names`) as tensors on `device` (default: the current CUDA
     device).  One vectored read moves them: blocks that no selected tensor touches are not fetched, and every touched block is
-    CRC-verified whole, including the bytes of unselected neighbours that share it.  Raises IOError when a block fails verification
-    and `verify` is set, SafetensorsError for a malformed header, KeyError for a name the file does not hold."""
+    CRC-verified whole, including the bytes of unselected neighbours that share it.  `slices` maps a name to (dim, start, stop): that
+    tensor comes back contiguous with shape[dim] = stop - start -- a tensor-parallel rank's shard, without the rest of the tensor ever
+    reaching HBM (see plan_ranges).  Raises IOError when a block fails verification and `verify` is set, SafetensorsError for a malformed
+    header, KeyError for a name the file does not hold, ValueError for a malformed slice (all before anything is allocated or read)."""
     import torch
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-    r = fs.open(path)
+    r, data_start, entries = _open_header(fs, path)
     try:
-        def read(off, n):
-            r.seek(off)
-            b = r.read_full(n)
-            if len(b) != n:
-                raise SafetensorsError("short read of the header: %d of %d bytes" % (len(b), n))
-            return b
-
-        data_start, entries = parse_header(read, r.len())
         selected = list(entries) if names is None else list(dict.fromkeys(names))
         for name in selected:
             if name not in entries:
                 raise KeyError("%s holds no tensor named %r" % (path, name))
+        plan = plan_ranges(data_start, entries, selected, slices)
         out, ranges = {}, []
-        for name in selected:
-            dtype, shape, begin, end = entries[name]
+        for name, dtype, shape, rng in plan:
             t = torch.empty(shape, dtype=dtype, device=dev)
             out[name] = t
-            if end > begin:
-                ranges.append((data_start + begin, end - begin, t.data_ptr()))
-        r.readv_device(ranges, torch.cuda.current_stream(dev).cuda_stream)
+            if rng is not None:
+                file_off, row_len, rows, file_pitch, dst_pitch = rng
+                ranges.append((file_off, row_len, rows, file_pitch, t.data_ptr(), dst_pitch))
+        r.readv_strided_device(ranges, torch.cuda.current_stream(dev).cuda_stream)
         _, bad, _ = r.verify()
         if verify and bad:
             raise IOError("%d blocks of %s failed CRC verification" % (bad, path))

@@ -19,7 +19,8 @@
  *   cv_fuse_read                 Reader::fuse_read                         reader.rs:101-124
  *   cv_seek / cv_pos / cv_len    Reader::seek / pos / len                  reader.rs:23-48, fs_reader.rs:109-126
  *   cv_close_reader              Reader::complete + drop                   java_abi.rs:157-166
- *   cv_read_device, cv_read_device_sharded, cv_read_many_device, cv_readv_device, cv_verify, cv_fuse_read_device
+ *   cv_read_device, cv_read_device_sharded, cv_read_many_device, cv_readv_device, cv_readv_strided_device, cv_verify,
+ *   cv_fuse_read_device
  *                                the CUDA counterpart the north_star adds behind the same reader handle
  *                                (no reference counterpart: the reference has no GPU code)
  * The cv_worker_* and cv_synth_* entry points are the test/bench fixture (the analogue of the reference's
@@ -133,6 +134,31 @@ int64_t cv_readv_device(cv_reader* r, const CvRange* ranges, int32_t n, cv_strea
  * *fetch_bytes = their summed length (what the read moves over PCIe).  Arrays may be NULL; cap = their length. */
 int64_t cv_readv_plan(cv_reader* r, const CvRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len,
                       int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes);
+/* Strided device read: cv_readv_device where a range is `rows` rows of `row_len` bytes -- a tensor-parallel rank's slice of a
+ * row-major tensor, for instance (dim 1 of [out, in]: one short piece of every row).  Row k is file bytes
+ * [file_off + k*file_pitch, +row_len) and lands at d_dst + k*dst_pitch.  Host work grows with the blocks the rows touch, not with the
+ * rows: every (range, touched block) pair plans into at most three spans, and spans of several rows are expanded into rows on the
+ * device (cvk_gather_strided).  Same verification and results as cv_readv_device (*nbytes = sum of rows * row_len, pos unchanged);
+ * rows == 0 or row_len == 0 ranges do nothing.  Errors (cv_last_error names the range): a negative row_len, rows or pitch; rows > 1
+ * with file_pitch or dst_pitch < row_len; (rows-1)*pitch + row_len overflowing int64; an extent
+ * [file_off, file_off + (rows-1)*file_pitch + row_len) outside the file; two ranges whose extents overlap -- which deliberately
+ * rejects interleaved strided ranges (rows of one range between rows of another): the slices of a safetensors file never need them;
+ * a destination whose first or last byte is not device memory on [b200] device; n < 0, or a NULL table with n > 0. */
+typedef struct CvStridedRange {
+    int64_t file_off;   /* first byte of row 0 in the file */
+    int64_t row_len;    /* bytes per row */
+    int64_t rows;
+    int64_t file_pitch; /* file distance between row starts (>= row_len when rows > 1) */
+    void* d_dst;        /* row k lands at d_dst + k * dst_pitch */
+    int64_t dst_pitch;  /* >= row_len when rows > 1 */
+} CvStridedRange;       /* 48 bytes */
+int64_t cv_readv_strided_device(cv_reader* r, const CvStridedRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes);
+/* The plan cv_readv_strided_device executes, as cv_readv_plan; a span now covers rows[i] rows of one range inside one block: bytes
+ * [block_off[i] + k*file_pitch, +len[i]) of the block for k < rows[i] (a plain range gives spans of one row).  A block is direct when
+ * its only span is one row that covers it whole. */
+int64_t cv_readv_strided_plan(cv_reader* r, const CvStridedRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len,
+                              int64_t* rows, int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks,
+                              int64_t* fetch_bytes);
 /* FUSE-shaped device read: seek(pos), read len bytes into HBM scratch, then scatter them into n_pages page
  * buffers (d_page_base + page_offsets[i], page_size each; last one partial) with the K3 gather kernel. */
 int64_t cv_fuse_read_device(cv_reader* r, int64_t pos, int64_t len, void* d_scratch, void* d_page_base,

@@ -16,7 +16,8 @@
  *                                                           curvine-common/src/fs/reader.rs:71-81
  *   cvk_gather_pages    Reader::fuse_read + as_iovec/writev curvine-common/src/fs/reader.rs:101-124,
  *                                                           curvine-fuse/src/session/fuse_response.rs:49-60,171-175
- *   cvk_pack_frames     RpcMessage::encode_protocol +       orpc/src/message/rpc_message.rs:301-311,
+ *   cvk_gather_strided  (no reference counterpart: the rows of tensor-parallel slices of a checkpoint, strided reads)
+ *   cvk_pack_frames     RpcMessage::encode_protocol +      orpc/src/message/rpc_message.rs:301-311,
  *                       RpcFrame::send/write_region          orpc/src/handler/rpc_frame.rs:97-121,205-220
  *                       (worker ReadHandler::read response)  curvine-server/src/worker/handler/read_handler.rs:143-183
  *   cvk_deinterleave_blocks, cvk_gather_shards_p2p  (no reference counterpart: model-distribution exchange, config C4)
@@ -97,6 +98,17 @@ typedef struct CvSeg {
     uint64_t len;
 } CvSeg;
 
+/* strided segment: rows equally spaced copies of len bytes,
+ * d_dst[dst_off + k*dst_pitch .. +len) = d_src[src_off + k*src_pitch .. +len) for k < rows */
+typedef struct CvStridedSeg {
+    uint64_t src_off;
+    uint64_t dst_off;
+    uint64_t len;
+    uint64_t rows;
+    uint64_t src_pitch;
+    uint64_t dst_pitch;
+} CvStridedSeg;
+
 /* Build the per-device constant tables (both polynomials).  Optional: every launcher does it lazily. */
 int cvk_init(int device);
 
@@ -130,6 +142,14 @@ int cvk_expand_streams(const CvStreamDesc* d_streams, uint32_t n_streams, CvFram
 int cvk_gather_pages(const uint8_t* d_src, const CvSeg* d_segs, uint32_t n, uint64_t total_bytes, uint8_t* d_dst,
                      cv_stream_t stream);
 
+/* K3 over 2D descriptors: every row of every segment, arbitrary alignment (rows of different segments must not overlap in d_dst).
+ * The rows are expanded into walker pieces on the device, in trains of at most 2^22 rows (cvk_tune(6, ...)), so the workspace
+ * does not grow with the row count.  Sizing the trains needs the row total: the launcher reads the n descriptors back, so it
+ * returns once the work queued on `stream` before it has finished (the copy itself stays asynchronous).
+ * total_bytes = sum of len * rows.  Algorithmic bytes: reads N, writes N. */
+int cvk_gather_strided(const uint8_t* d_src, const CvStridedSeg* d_segs, uint32_t n, uint64_t total_bytes, uint8_t* d_dst,
+                       cv_stream_t stream);
+
 /* K4: worker-side inverse of K2.  For frame f: write the 22-byte prefix (+ no header) at
  * d_wire + d_desc[f].wire_off, copy d_src[dst_off .. +data_len) behind it, and CRC the source bytes
  * (d_block_crc as in K2; may be NULL).  Algorithmic bytes: reads N, writes N + 22F. */
@@ -162,7 +182,8 @@ int cvk_profile_collect(double* walk_ms_total, uint32_t* walk_launches);
  * {2,4}; what 3: shared-memory staged (cp.async) DST walks (1) or register-tiled ones (0, default; CVK_STAGED=1 in the
  * environment flips the default); what 4: segment size 2^value bytes
  * (12..20) for every launcher instead of the size-derived choice, 0 = back to automatic; what 5: 0 routes inputs of at most ~1 MiB through the general launch train
- * instead of the single-launch small-input kernels (default 1).  Process-wide; results are identical for every setting (tools/kbench.py sweeps it). */
+ * instead of the single-launch small-input kernels (default 1); what 6: rows per train of cvk_gather_strided, 1..2^22, 0 = back to
+ * the default 2^22.  Process-wide; results are identical for every setting (tools/kbench.py sweeps it). */
 int cvk_tune(int what, int value);
 
 /* Number of kernel launches issued by this library in this process (bench.py's gpu_launches claim). */
