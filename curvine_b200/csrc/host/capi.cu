@@ -353,6 +353,15 @@ static std::vector<ReadvRange> strided_ranges(const CvStridedRange* ranges, int3
     return out;
 }
 
+static std::vector<ReadvRange> cast_ranges(const CvCastRange* ranges, int32_t n) {
+    std::vector<ReadvRange> out;
+    for (int32_t i = 0; ranges && i < n; i++) {
+        const CvCastRange& s = ranges[i];
+        out.push_back(ReadvRange{s.file_off, s.row_len, static_cast<uint8_t*>(s.d_dst), s.rows, s.file_pitch, s.dst_pitch, s.src_dtype, s.dst_dtype});
+    }
+    return out;
+}
+
 static int64_t readv_device_common(cv_reader* r, const std::vector<ReadvRange>& rs, int32_t n, cv_stream_t stream, int64_t* nbytes) {
     API_TRY(ensure_dev(r));
     int64_t got = 0;
@@ -422,6 +431,24 @@ int64_t cv_readv_strided_plan(cv_reader* r, const CvStridedRange* ranges, int32_
     API_NEED(r);
     if (n > 0) API_NEED(ranges);
     return readv_plan_common(r, strided_ranges(ranges, n), n, block_index, block_off, len, rows, range_index, direct, cap, n_spans, n_blocks, fetch_bytes);
+    API_GUARD_END
+}
+
+int64_t cv_readv_cast_device(cv_reader* r, const CvCastRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes) {
+    API_GUARD_BEGIN
+    API_NEED(r);
+    API_NEED(nbytes);
+    if (n > 0) API_NEED(ranges);
+    return readv_device_common(r, cast_ranges(ranges, n), n, stream, nbytes);
+    API_GUARD_END
+}
+
+int64_t cv_readv_cast_plan(cv_reader* r, const CvCastRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len, int64_t* rows,
+                           int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes) {
+    API_GUARD_BEGIN
+    API_NEED(r);
+    if (n > 0) API_NEED(ranges);
+    return readv_plan_common(r, cast_ranges(ranges, n), n, block_index, block_off, len, rows, range_index, direct, cap, n_spans, n_blocks, fetch_bytes);
     API_GUARD_END
 }
 
@@ -901,6 +928,11 @@ int64_t cv_synth_create_file(cv_worker* w, const char* path, int64_t inode_id, i
 // launchers that existed before this one).  There this weak definition keeps the symbol resolvable and reports the strided gather as
 // unsupported; it copies nothing.  Every library that links kernels.cu gets the kernel: the strong definition there replaces this one.
 __attribute__((weak)) int cvk_gather_strided(const uint8_t*, const CvStridedSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) {
+    return n ? int(cudaErrorNotSupported) : 0;
+}
+
+// The same for the cast gather of cast reads (cv_readv_cast_device).
+__attribute__((weak)) int cvk_gather_cast(const uint8_t*, const CvCastSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) {
     return n ? int(cudaErrorNotSupported) : 0;
 }
 

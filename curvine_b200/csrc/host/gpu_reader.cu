@@ -351,6 +351,29 @@ Err GpuFsReader::read_device_sharded(int rank, int world, void* d_dst, int64_t c
     return Err::ok();
 }
 
+static int64_t dtype_size(int32_t dt) { return dt == CV_DTYPE_F32 ? 4 : dt == CV_DTYPE_NONE ? 1 : 2; }
+
+// A range's destination row in bytes: row_len converted to the destination element size.
+static int64_t dst_row_len(const ReadvRange& r) { return r.cast() ? r.row_len / dtype_size(r.src_dtype) * dtype_size(r.dst_dtype) : r.row_len; }
+
+// The rules only a converting range has (plan_readv)
+static Err check_cast(const FileBlocks& fb, const ReadvRange& r, int32_t i) {
+    for (int32_t dt : {r.src_dtype, r.dst_dtype})
+        if (dt < CV_DTYPE_NONE || dt > CV_DTYPE_BF16) return Err::common(str_printf("readv: range %d has an unknown dtype code %d", i, dt));
+    if (!r.cast()) return Err::ok();
+    if (r.src_dtype == CV_DTYPE_NONE || r.dst_dtype == CV_DTYPE_NONE)
+        return Err::common(str_printf("readv: range %d converts dtype %d to %d: conversions are between F32, F16 and BF16 only", i, r.src_dtype, r.dst_dtype));
+    const int64_t ss = dtype_size(r.src_dtype), ds = dtype_size(r.dst_dtype);
+    if (r.file_off % ss || r.row_len % ss || (r.rows > 1 && r.file_pitch % ss))
+        return Err::common(str_printf("readv: range %d: file_off, row_len and file_pitch must be multiples of the source element size (%lld)", i, (long long)ss));
+    if (reinterpret_cast<uintptr_t>(r.dst) % ds || (r.rows > 1 && r.dst_pitch % ds))
+        return Err::common(str_printf("readv: range %d: the destination and dst_pitch must be multiples of the destination element size (%lld)", i, (long long)ds));
+    if (fb.status.block_size % ss)
+        return Err::common(str_printf("readv: range %d: the file's block size %lld is not a multiple of the source element size (%lld)", i,
+                                      (long long)fb.status.block_size, (long long)ss));
+    return Err::ok();
+}
+
 Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::vector<ReadvBlock>* blocks, std::vector<ReadvSpan>* spans) {
     blocks->clear(), spans->clear();
     if (n < 0) return Err::common(str_printf("readv: negative range count %d", n));
@@ -363,12 +386,14 @@ Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::v
         if (r.row_len < 0) return Err::common(str_printf("readv: range %d has a negative length (%lld)", i, (long long)r.row_len));
         if (r.rows < 0) return Err::common(str_printf("readv: range %d has a negative row count (%lld)", i, (long long)r.rows));
         if (r.file_pitch < 0 || r.dst_pitch < 0) return Err::common(str_printf("readv: range %d has a negative pitch", i));
-        if (r.rows > 1 && (r.file_pitch < r.row_len || r.dst_pitch < r.row_len))
+        CV_RETURN_IF_ERR(check_cast(fb, r, i));
+        const int64_t dst_row = dst_row_len(r);
+        if (r.rows > 1 && (r.file_pitch < r.row_len || r.dst_pitch < dst_row))
             return Err::common(str_printf("readv: range %d has a pitch shorter than its row length (%lld)", i, (long long)r.row_len));
         int64_t& ext = extent[static_cast<size_t>(i)];
         ext = r.rows == 0 ? 0 : r.row_len;
         for (int64_t pitch : {r.file_pitch, r.dst_pitch})
-            if (r.rows > 1 && pitch > 0 && r.rows - 1 > (INT64_MAX - r.row_len) / pitch)
+            if (r.rows > 1 && pitch > 0 && r.rows - 1 > (INT64_MAX - std::max(r.row_len, dst_row)) / pitch)
                 return Err::common(str_printf("readv: range %d: (rows - 1) * pitch + row_len overflows", i));
         if (r.rows > 1) ext += (r.rows - 1) * r.file_pitch;
         if (r.file_off < 0 || r.file_off > flen || ext > flen - r.file_off)
@@ -382,6 +407,8 @@ Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::v
     for (int32_t i : order) {
         const ReadvRange& r = ranges[i];
         const int64_t L = r.row_len, R = r.rows, P = R > 1 ? r.file_pitch : L, off = r.file_off;
+        // a converting range's in-row offsets scale to destination bytes; its row offsets are dst_pitch apart as for any range
+        const int64_t ss = r.cast() ? dtype_size(r.src_dtype) : 1, ds = r.cast() ? dtype_size(r.dst_dtype) : 1;
         // next byte to place: column `col` of row `row`.  Every pass of the loop handles one touched block, in file order.
         int64_t row = 0, col = 0;
         while (row < R) {
@@ -391,15 +418,19 @@ Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::v
             CV_RETURN_IF_ERR(fb.get_read_block(q, &boff, &idx));
             const int64_t bs = q - boff, be = bs + fb.block_locs[idx].block.len;
             if (blocks->empty() || blocks->back().block != idx) blocks->push_back(ReadvBlock{idx, false, spans->size(), 0});
+            Err bad;
             auto emit = [&](int64_t at, int64_t len, int64_t rows, int64_t dst_off) {
+                if (((at - off) | len) % ss)  // only a file whose blocks are not all block_size long gets here
+                    bad = Err::common(str_printf("readv: range %d: an element straddles the edge of block %zu", i, idx));
                 spans->push_back(ReadvSpan{at - bs, len, rows, dst_off, i});
                 blocks->back().n_spans++;
             };
             // the row in progress, when it began in an earlier block or runs past this one: clipped by the block's edge
             if (col > 0 || off + row * P + L > be) {
                 const int64_t take = std::min(L - col, be - q);
-                emit(q, take, 1, row * r.dst_pitch + col);
+                emit(q, take, 1, row * r.dst_pitch + col / ss * ds);
                 col += take;
+                if (bad) return bad;
                 if (col < L) continue;  // it goes on in the next block
                 row++, col = 0;
             }
@@ -415,12 +446,13 @@ Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::v
                 emit(off + row * P, take, 1, row * r.dst_pitch);
                 col = take;
             }
+            if (bad) return bad;
             // otherwise the next row starts in a later block: the next pass looks that block up directly
         }
     }
     for (ReadvBlock& b : *blocks) {
         const ReadvSpan& s = (*spans)[b.first_span];
-        b.direct = b.n_spans == 1 && s.rows == 1 && s.block_off == 0 && s.len == fb.block_locs[b.block].block.len;
+        b.direct = b.n_spans == 1 && s.rows == 1 && s.block_off == 0 && s.len == fb.block_locs[b.block].block.len && !ranges[s.range].cast();
     }
     return Err::ok();
 }
@@ -592,17 +624,18 @@ static Err check_device_dst(const void* p, int device) {
 enum JobMode : uint8_t { kPlain = 0, kFramed = 1, kHole = 3 };
 
 // Layout of the per-call device tables (shared by all readers of the context) and of their pinned host image:
-//   off[J] len[J] expect[J] skip[J] | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F] | segs[n_segs] | strided[n_strided]
+//   off[J] len[J] expect[J] skip[J] | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F] | segs[n_segs] | strided[n_strided] | casts[n_casts]
 // off .. skip are uploaded before the fetch starts; crc .. ferr are the results copied back.
 struct TableLayout {
-    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, o_segs = 0, o_strided = 0, bytes = 0;
+    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, o_segs = 0, o_strided = 0, o_casts = 0, bytes = 0;
     TableLayout() = default;
-    TableLayout(size_t j, size_t f, size_t n_segs, size_t n_strided) : J(j), F(f) {
+    TableLayout(size_t j, size_t f, size_t n_segs, size_t n_strided, size_t n_casts) : J(j), F(f) {
         auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
         o_len = up(8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_crc = up(o_skip + J);
         o_streams = up(o_crc + 4 * res_words()), o_fdesc = up(o_streams + sizeof(CvStreamDesc) * J);
         o_segs = up(o_fdesc + sizeof(CvFrameDesc) * F), o_strided = up(o_segs + sizeof(CvSeg) * n_segs);
-        bytes = up(o_strided + sizeof(CvStridedSeg) * n_strided);
+        o_casts = up(o_strided + sizeof(CvStridedSeg) * n_strided);
+        bytes = up(o_casts + sizeof(CvCastSeg) * n_casts);
     }
     size_t res_words() const { return J + 4 + F; }
     uint64_t* off(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t); }
@@ -615,6 +648,7 @@ struct TableLayout {
     CvFrameDesc* fdesc(uint8_t* t) const { return reinterpret_cast<CvFrameDesc*>(t + o_fdesc); }
     CvSeg* segs(uint8_t* t) const { return reinterpret_cast<CvSeg*>(t + o_segs); }
     CvStridedSeg* strided(uint8_t* t) const { return reinterpret_cast<CvStridedSeg*>(t + o_strided); }
+    CvCastSeg* casts(uint8_t* t) const { return reinterpret_cast<CvCastSeg*>(t + o_casts); }
 };
 
 // What one run_jobs call does, decided before any CUDA call.
@@ -634,7 +668,7 @@ struct GpuFsReader::CallPlan {
     TableLayout tl;
 };
 
-Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, CallPlan* out) const {
+Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, size_t n_casts, CallPlan* out) const {
     CallPlan& P = *out;
     const B200Conf& bc = ctx_->conf.b200;
     const size_t J = jobs.size();
@@ -680,7 +714,7 @@ Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n
     P.group_verbatim.assign(P.NG, 0);
     for (size_t j = 0; j < J; j++) P.group_verbatim[j / P.k] |= P.mode[j] == kFramed;
     P.T_threads = static_cast<int>(std::min<size_t>(static_cast<size_t>(std::max(1, bc.fetch_threads)), P.NG));
-    P.tl = TableLayout(J, P.F, n_segs, n_strided);
+    P.tl = TableLayout(J, P.F, n_segs, n_strided, n_casts);
     return Err::ok();
 }
 
@@ -1032,10 +1066,10 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     CU_TRY(cudaStreamWaitEvent(G.vstream, G.entry_ev, 0));
     const B200Conf& bc = ctx_->conf.b200;
     const int poly = bc.verify_poly ? 1 : 0;
-    const size_t n_segs = pages ? pages->segs.size() : 0, n_strided = pages ? pages->strided.size() : 0;
+    const size_t n_segs = pages ? pages->segs.size() : 0, n_strided = pages ? pages->strided.size() : 0, n_casts = pages ? pages->casts.size() : 0;
 
     CallPlan P;
-    CV_RETURN_IF_ERR(plan_call(jobs, n_segs, n_strided, &P));
+    CV_RETURN_IF_ERR(plan_call(jobs, n_segs, n_strided, n_casts, &P));
     Call c(*this, jobs, P, d_dst);
     if (!(bc.zero_copy && !P.call_framed)) CV_RETURN_IF_ERR(c.ensure_ring());
 
@@ -1070,6 +1104,10 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     if (n_strided) {  // and so does its table of strided segments
         memcpy(tl.strided(h), pages->strided.data(), sizeof(CvStridedSeg) * n_strided);
         CU_TRY(cudaMemcpyAsync(tl.strided(T), tl.strided(h), sizeof(CvStridedSeg) * n_strided, cudaMemcpyHostToDevice, G.vstream));
+    }
+    if (n_casts) {  // and its table of cast segments
+        memcpy(tl.casts(h), pages->casts.data(), sizeof(CvCastSeg) * n_casts);
+        CU_TRY(cudaMemcpyAsync(tl.casts(T), tl.casts(h), sizeof(CvCastSeg) * n_casts, cudaMemcpyHostToDevice, G.vstream));
     }
     CU_TRY(cudaMemsetAsync(tl.crc(T), 0, 4 * tl.res_words(), G.vstream));
     CvStreamDesc* sd = tl.streams(h);
@@ -1148,6 +1186,8 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
         CVK_TRY(cvk_gather_pages(d_dst, tl.segs(T), static_cast<uint32_t>(n_segs), pages->total, pages->d_out, G.vstream));
     if (n_strided)  // spans of several rows each
         CVK_TRY(cvk_gather_strided(d_dst, tl.strided(T), static_cast<uint32_t>(n_strided), pages->strided_total, pages->d_out, G.vstream));
+    if (n_casts)  // spans of converting ranges: K5 out of the verified staging
+        CVK_TRY(cvk_gather_cast(d_dst, tl.casts(T), static_cast<uint32_t>(n_casts), pages->cast_elems, pages->d_out, G.vstream));
     CU_TRY(cudaMemcpyAsync(G.h_result, d_crc, 4 * tl.res_words(), cudaMemcpyDeviceToHost, G.vstream));
     CU_TRY(cudaEventRecord(G.done_ev, G.vstream));
     CU_TRY(cudaStreamWaitEvent(static_cast<cudaStream_t>(user_stream), G.done_ev, 0));
@@ -1209,9 +1249,10 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
         const ReadvRange& r = ranges[i];
         if (r.row_len == 0 || r.rows == 0) continue;
         CV_RETURN_IF_ERR(check_device_dst(r.dst, G.device).ctx(str_printf("range %d", i)));
-        CV_RETURN_IF_ERR(check_device_dst(r.dst + (r.rows - 1) * r.dst_pitch + r.row_len - 1, G.device).ctx(str_printf("range %d (last byte)", i)));
+        const int64_t dst_row = dst_row_len(r);
+        CV_RETURN_IF_ERR(check_device_dst(r.dst + (r.rows - 1) * r.dst_pitch + dst_row - 1, G.device).ctx(str_printf("range %d (last byte)", i)));
         lo = std::min(lo, reinterpret_cast<uintptr_t>(r.dst));
-        total += r.rows * r.row_len;
+        total += r.rows * dst_row;
     }
     if (blocks.empty()) return Err::ok();
     std::vector<size_t> boundary;
@@ -1246,18 +1287,24 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
             jobs.push_back(Job{&fb.block_locs[b.block], 0, fb.block_locs[b.block].block.len, at, true});
             for (size_t k = b.first_span; k < b.first_span + b.n_spans; k++) {
                 const ReadvSpan& s = spans[k];
+                const ReadvRange& r = ranges[s.range];
                 const uint64_t src = static_cast<uint64_t>(at + s.block_off), dst = static_cast<uint64_t>(dst_of(s)), len = static_cast<uint64_t>(s.len);
-                if (s.rows == 1) {
+                if (r.cast()) {
+                    const uint64_t elems = len / static_cast<uint64_t>(dtype_size(r.src_dtype)), rows = static_cast<uint64_t>(s.rows);
+                    sc.casts.push_back(CvCastSeg{src, dst, elems, rows, static_cast<uint64_t>(r.file_pitch), static_cast<uint64_t>(r.dst_pitch),
+                                                 sc.cast_chunks, r.src_dtype, r.dst_dtype});
+                    sc.cast_elems += elems * rows;
+                    sc.cast_chunks += rows * CV_CAST_ROW_CHUNKS(elems);
+                } else if (s.rows == 1) {
                     sc.segs.push_back(CvSeg{src, dst, len});
                     sc.total += len;
                 } else {
-                    const ReadvRange& r = ranges[s.range];
                     sc.strided.push_back(CvStridedSeg{src, dst, len, static_cast<uint64_t>(s.rows), static_cast<uint64_t>(r.file_pitch), static_cast<uint64_t>(r.dst_pitch)});
                     sc.strided_total += len * static_cast<uint64_t>(s.rows);
                 }
             }
         }
-        CV_RETURN_IF_ERR(run_jobs(jobs, base, stream, sc.segs.empty() && sc.strided.empty() ? nullptr : &sc));
+        CV_RETURN_IF_ERR(run_jobs(jobs, base, stream, sc.segs.empty() && sc.strided.empty() && sc.casts.empty() ? nullptr : &sc));
         jobs.clear();
     } while (next < boundary.size());
     *n = total;

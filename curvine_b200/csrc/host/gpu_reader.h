@@ -50,16 +50,20 @@ Err plan_shard(const FileBlocks& fb, int rank, int world, int64_t cap, std::vect
 // [file_off + k*file_pitch, +row_len) and lands at dst + k*dst_pitch (a plain byte range is one row).  The plan lists every block a range
 // touches, in file order, with the spans of it that go to which range.  A block is direct when one span of one row covers all of it: it
 // lands in place as an ordinary whole-block job.  Every other touched block is a boundary block: it is fetched whole into device staging,
-// verified there like any whole block, and its spans are delivered from the staging by K3.
+// verified there like any whole block, and its spans are delivered from the staging by K3.  A range whose src_dtype differs from its
+// dst_dtype converts its elements (CV_DTYPE_*): its file side is in source bytes, its destination side (dst, dst_pitch, a span's dst_off)
+// in destination bytes, and none of the blocks it touches is direct, so each is verified before K5 converts it out of the staging.
 struct ReadvRange {
     int64_t file_off, row_len;
     uint8_t* dst;
     int64_t rows = 1, file_pitch = 0, dst_pitch = 0;  // the pitches only matter when rows > 1
+    int32_t src_dtype = CV_DTYPE_NONE, dst_dtype = CV_DTYPE_NONE;
+    bool cast() const { return src_dtype != dst_dtype; }
 };
 struct ReadvSpan {
     int64_t block_off, len;  // row k < rows of the span: bytes [block_off + k*file_pitch, +len) of the block
     int64_t rows;
-    int64_t dst_off;         // row k goes to ranges[range].dst + dst_off + k*dst_pitch
+    int64_t dst_off;         // row k goes to ranges[range].dst + dst_off + k*dst_pitch (destination bytes)
     int32_t range;
 };
 struct ReadvBlock {
@@ -70,7 +74,10 @@ struct ReadvBlock {
 // Ranges may come in any order.  An error: a negative row_len, rows or pitch; rows > 1 with a pitch shorter than row_len; an extent
 // [file_off, file_off + (rows-1)*file_pitch + row_len) outside the file (or one that overflows); two ranges whose extents overlap in the
 // file -- interleaved strided ranges included.  For one range and one block the rows that meet the block form at most three spans (a
-// clipped first row, the whole rows, a clipped last row), computed without visiting the rows: O(ranges + touched blocks).
+// clipped first row, the whole rows, a clipped last row), computed without visiting the rows: O(ranges + touched blocks).  A converting
+// range is an error besides when a dtype code is unknown, when it converts to or from CV_DTYPE_NONE, when an element could straddle two
+// blocks or a source or destination element is misaligned (see cv_readv_cast_device), or when its dst_pitch is shorter than its
+// destination row.
 Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::vector<ReadvBlock>* blocks, std::vector<ReadvSpan>* spans);
 
 class GpuIngest;  // per-FsContext pinned ring + streams
@@ -94,7 +101,7 @@ class GpuFsReader {
     // block_size bytes (slot j = block j*world + rank).  *n = bytes landed (sum of those block lengths).
     Err read_device_sharded(int rank, int world, void* d_dst, int64_t cap, void* stream, int64_t* n);
     // Vectored read (plan_readv): every touched block is fetched once and its CRC compared over the whole block.  Ordered on `stream`
-    // when the call returns; does not move pos.  *n = sum of rows * row_len.
+    // when the call returns; does not move pos.  *n = bytes delivered: sum of rows * row_len (converted to destination bytes).
     Err readv_device(const ReadvRange* ranges, int32_t n_ranges, void* stream, int64_t* n);
     // Waits for outstanding work; sum_crc = u64 sum of the per-block CRCs computed so far (verify_poly),
     // n_bad = blocks whose CRC differed from the manifest.
@@ -118,17 +125,19 @@ class GpuFsReader {
     // scatter riding on a read: after the bytes landed in d_dst and were CRC'd, segs[i] copies d_dst + src_off to d_out + dst_off
     // (K3), in the same launch train, no extra sync.  Page buffers of a FUSE reply (Reader::fuse_read + ResponseData::as_iovec on the
     // device), or the spans of the boundary blocks of a vectored read: one-row spans as segs (K3), spans of several rows as strided
-    // (K3 over 2D descriptors).
+    // (K3 over 2D descriptors), spans of converting ranges as casts (K5).
     struct Scatter {
         uint8_t* d_out = nullptr;
         std::vector<CvSeg> segs;
         uint64_t total = 0;  // sum of segs[i].len
         std::vector<CvStridedSeg> strided;
         uint64_t strided_total = 0;  // sum of strided[i].len * strided[i].rows
+        std::vector<CvCastSeg> casts;
+        uint64_t cast_elems = 0, cast_chunks = 0;  // sum of casts[i].elems * rows, and the next segment's `first`
     };
     struct CallPlan;  // what one run_jobs call does, decided up front (plan_call)
     struct Call;      // one run_jobs call in flight: fetch workers and the ingest paths of a copy group
-    Err plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, CallPlan* out) const;
+    Err plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, size_t n_casts, CallPlan* out) const;
     Err run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* stream, const Scatter* scatter = nullptr);
     Err read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const Scatter* scatter);
     FsContext* ctx_ = nullptr;

@@ -931,6 +931,135 @@ __global__ void verify_crcs_kernel(const uint32_t* crc, const uint32_t* expect, 
     if ((threadIdx.x & 31) == 0 && m) atomicAdd(n_bad, __popc(m));
 }
 
+// ------------------------------------------------------------------ K5: gather with a dtype conversion
+// The conversions are integer arithmetic on the bit patterns (no FP state, no intrinsics), IEEE round-to-nearest-even.
+
+__device__ __forceinline__ uint32_t f16_to_f32(uint32_t h) {  // exact
+    const uint32_t sign = (h & 0x8000u) << 16, e = (h >> 10) & 0x1fu;
+    uint32_t m = h & 0x3ffu;
+    if (e == 0x1fu) return sign | 0x7f800000u | (m << 13);  // inf, NaN (payload kept)
+    if (e) return sign | ((e + 112u) << 23) | (m << 13);
+    if (!m) return sign;
+    uint32_t k = 0;  // subnormal m * 2^-24: normalise, 2^(-14-k) with k the shifts that bring the top bit to bit 10
+    while (!(m & 0x400u)) m <<= 1, k++;
+    return sign | ((113u - k) << 23) | ((m & 0x3ffu) << 13);
+}
+
+__device__ __forceinline__ uint32_t f32_to_f16(uint32_t u) {
+    const uint32_t sign = (u >> 16) & 0x8000u, a = u & 0x7fffffffu;
+    if (a > 0x7f800000u) return sign | 0x7e00u;  // NaN
+    if (a >= 0x477ff000u) return sign | 0x7c00u;  // |x| >= 65520 (halfway above the largest half, 65504): inf
+    if (a >= 0x38800000u) {                       // normal half: rebias the exponent, round the 13 dropped bits
+        const uint32_t h = (a - 0x38000000u) >> 13, r = a & 0x1fffu;
+        return sign | (h + (r > 0x1000u || (r == 0x1000u && (h & 1u))));
+    }
+    if (a <= 0x33000000u) return sign;  // |x| <= 2^-25, half the smallest subnormal: ties to the even zero
+    const uint32_t s = 126u - (a >> 23), m = (a & 0x7fffffu) | 0x800000u;  // subnormal half: x / 2^-24 = m >> s, s in [14, 24]
+    const uint32_t h = m >> s, r = m & ((1u << s) - 1u), half = 1u << (s - 1u);
+    return sign | (h + (r > half || (r == half && (h & 1u))));  // a carry into bit 10 is the smallest normal: still right
+}
+
+__device__ __forceinline__ uint32_t f32_to_bf16(uint32_t u) {
+    if ((u & 0x7fffffffu) > 0x7f800000u) return (u >> 16) | 0x40u;  // NaN: quiet, sign and top payload bits kept
+    return (u + 0x7fffu + ((u >> 16) & 1u)) >> 16;                  // overflow carries into the exponent: inf
+}
+
+__device__ __forceinline__ uint32_t cast_size(int32_t dt) { return dt == CV_DTYPE_F32 ? 4u : 2u; }
+
+__device__ __forceinline__ uint32_t cast_elem(uint32_t v, int32_t sdt, int32_t ddt) {
+    if (sdt == ddt) return v;
+    const uint32_t f = sdt == CV_DTYPE_F16 ? f16_to_f32(v) : sdt == CV_DTYPE_BF16 ? v << 16 : v;
+    return ddt == CV_DTYPE_F16 ? f32_to_f16(f) : ddt == CV_DTYPE_BF16 ? f32_to_bf16(f) : f;
+}
+
+__device__ __forceinline__ uint32_t ld_elem(const uint8_t* p, uint32_t size) {
+    return size == 4 ? *reinterpret_cast<const uint32_t*>(p) : *reinterpret_cast<const uint16_t*>(p);
+}
+
+__device__ __forceinline__ void st_elem(uint8_t* p, uint32_t size, uint32_t v) {
+    if (size == 4) *reinterpret_cast<uint32_t*>(p) = v;
+    else *reinterpret_cast<uint16_t*>(p) = static_cast<uint16_t>(v);
+}
+
+// 8 source elements from p (aligned to the element size only), in the widest loads the address allows
+__device__ __forceinline__ void ld_chunk(const uint8_t* p, uint32_t size, uint32_t v[8]) {
+    const uint32_t a = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(p)) & 15u;
+    if (size == 4 && a == 0) {
+        const uint4 x = ld_plain(reinterpret_cast<const uint4*>(p)), y = ld_plain(reinterpret_cast<const uint4*>(p + 16));
+        v[0] = x.x, v[1] = x.y, v[2] = x.z, v[3] = x.w, v[4] = y.x, v[5] = y.y, v[6] = y.z, v[7] = y.w;
+    } else if (size == 4 && (a & 7u) == 0) {
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const uint64_t w = reinterpret_cast<const uint64_t*>(p)[k];
+            v[2 * k] = static_cast<uint32_t>(w), v[2 * k + 1] = static_cast<uint32_t>(w >> 32);
+        }
+    } else if (size == 2 && a == 0) {
+        const uint4 x = ld_plain(reinterpret_cast<const uint4*>(p));
+        const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+        for (int k = 0; k < 4; k++) v[2 * k] = w[k] & 0xffffu, v[2 * k + 1] = w[k] >> 16;
+    } else if (size == 2 && (a & 3u) == 0) {
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const uint32_t w = reinterpret_cast<const uint32_t*>(p)[k];
+            v[2 * k] = w & 0xffffu, v[2 * k + 1] = w >> 16;
+        }
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; k++) v[k] = ld_elem(p + k * size, size);
+    }
+}
+
+// Grid-stride over the work chunks of all segments (CvCastSeg::first numbers them): neighbouring threads take neighbouring chunks, so
+// every load and store of a warp is coalesced whatever the shape.  In a row whose destination is `head` elements short of a 16-byte
+// boundary, chunk 0 holds those head elements and chunk k >= 1 the 8 elements from head + 8(k-1) on (with head = 0, chunk k holds 8k..):
+// every whole chunk stores one (2-byte destination) or two (4-byte destination) aligned 16-byte vectors.
+__global__ void __launch_bounds__(256) gather_cast_kernel(const uint8_t* __restrict__ src, const CvCastSeg* __restrict__ segs, uint32_t n,
+                                                          uint8_t* __restrict__ dst) {
+    const uint64_t total = segs[n - 1].first + segs[n - 1].rows * CV_CAST_ROW_CHUNKS(segs[n - 1].elems);
+    uint32_t d = 0;  // the segment of the previous chunk: chunks only grow, so the search starts there
+    for (uint64_t c = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; c < total; c += uint64_t(gridDim.x) * blockDim.x) {
+        if (d + 1 < n && segs[d + 1].first <= c) {  // the last segment whose first chunk is <= c (empty segments share their first)
+            uint32_t lo = d + 1, hi = n - 1;
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi + 1) >> 1;
+                if (segs[mid].first <= c) lo = mid;
+                else hi = mid - 1;
+            }
+            d = lo;
+        }
+        const CvCastSeg& s = segs[d];
+        const uint64_t cpr = CV_CAST_ROW_CHUNKS(s.elems), rel = c - s.first;
+        if (c < s.first || rel >= s.rows * cpr) continue;  // a table whose `first` leaves gaps: nothing is written outside a row
+        const int32_t sdt = s.src_dtype, ddt = s.dst_dtype;
+        if ((sdt != CV_DTYPE_F32 && sdt != CV_DTYPE_F16 && sdt != CV_DTYPE_BF16) || (ddt != CV_DTYPE_F32 && ddt != CV_DTYPE_F16 && ddt != CV_DTYPE_BF16))
+            continue;
+        const uint32_t ss = cast_size(sdt), ds = cast_size(ddt);
+        const uint64_t row = rel < cpr ? 0 : rel / cpr, k = rel - row * cpr;
+        const uint8_t* sp = src + s.src_off + row * s.src_pitch;
+        uint8_t* dp = dst + s.dst_off + row * s.dst_pitch;
+        const uint32_t head = ((16u - (static_cast<uint32_t>(reinterpret_cast<uintptr_t>(dp)) & 15u)) & 15u) / ds;
+        const int64_t e0 = 8 * int64_t(k) - int64_t((8u - head) & 7u);  // chunk k: elements [e0, e0 + 8) of the row, clipped to it
+        const int64_t lo = e0 > 0 ? e0 : 0, hi = e0 + 8 < int64_t(s.elems) ? e0 + 8 : int64_t(s.elems);
+        if (lo >= hi) continue;
+        if (hi - lo == 8) {  // a whole chunk: its destination is 16-byte aligned
+            uint32_t v[8];
+            ld_chunk(sp + lo * ss, ss, v);
+#pragma unroll
+            for (int j = 0; j < 8; j++) v[j] = cast_elem(v[j], sdt, ddt);
+            uint4* o = reinterpret_cast<uint4*>(dp + lo * ds);
+            if (ds == 2) {
+                st_vec(o, make_uint4(v[0] | v[1] << 16, v[2] | v[3] << 16, v[4] | v[5] << 16, v[6] | v[7] << 16));
+            } else {
+                st_vec(o, make_uint4(v[0], v[1], v[2], v[3]));
+                st_vec(o + 1, make_uint4(v[4], v[5], v[6], v[7]));
+            }
+        } else {
+            for (int64_t e = lo; e < hi; e++) st_elem(dp + e * ds, ds, cast_elem(ld_elem(sp + e * ss, ss), sdt, ddt));
+        }
+    }
+}
+
 // ------------------------------------------------------------------ host side
 
 static std::atomic<uint64_t> g_launches{0};
@@ -1109,12 +1238,12 @@ static void launch_expand(const Workspace& w, uint32_t n, uint32_t seg_shift, cu
 
 static void launch_walk_crc_dst(int dev, cudaStream_t st, const Workspace& w, uint32_t n, const CrcConsts* cc) {
     const dim3 grid(g_sm_count[dev]), block(1024);
-    if (g_staged.load(std::memory_order_relaxed))
+    if (g_staged.load(std::memory_order_relaxed)) {
         walk_kernel<true, true, 4, kStageCrc><<<grid, block, kSmemBytes + kStageCrc * 512 * 32, st>>>(CV_WALK_ARGS);
-    else if (g_tile_crc_dst.load(std::memory_order_relaxed) == 2)
-        walk_kernel<true, true, 2><<<grid, block, kSmemBytes, st>>>(CV_WALK_ARGS);
-    else
-        walk_kernel<true, true, 4><<<grid, block, kSmemBytes, st>>>(CV_WALK_ARGS);
+    } else {  // the register-tiled walks differ only in rows per tile: one launch of the chosen instance
+        auto walk = g_tile_crc_dst.load(std::memory_order_relaxed) == 2 ? walk_kernel<true, true, 2> : walk_kernel<true, true, 4>;
+        walk<<<grid, block, kSmemBytes, st>>>(CV_WALK_ARGS);
+    }
 }
 
 // copy-only walk: no shared memory, one CTA per SM (the kernels need > 32 registers, so two 1024-thread CTAs never fit).
@@ -1357,6 +1486,19 @@ int cvk_gather_strided(const uint8_t* d_src, const CvStridedSeg* d_segs, uint32_
     }
     const cudaError_t freed = cudaFreeAsync(d_pref, st);
     return rc ? rc : int(freed);
+}
+
+int cvk_gather_cast(const uint8_t* d_src, const CvCastSeg* d_segs, uint32_t n, uint64_t total_elems, uint8_t* d_dst, cv_stream_t stream) {
+    if (n == 0 || total_elems == 0) return 0;
+    DeviceGuard guard(d_dst);
+    int dev;
+    if (int rc = ensure_device(&dev)) return rc;
+    // the table stays on the device: the kernel takes the chunk count from its last entry.  One thread per 8 elements, at most 8
+    // CTAs of 256 per SM; the grid-stride loop takes the rest (and the head chunks of many short rows).
+    const uint64_t want = total_elems / (8 * 256) + 1, cap = uint64_t(g_sm_count[dev]) * 8;
+    gather_cast_kernel<<<uint32_t(want < cap ? want : cap), 256, 0, static_cast<cudaStream_t>(stream)>>>(d_src, d_segs, n, d_dst);
+    count_launch();
+    return int(cudaGetLastError());
 }
 
 int cvk_deinterleave_blocks(const uint8_t* d_gathered, uint64_t shard_stride, uint32_t world, uint64_t block_size,

@@ -236,6 +236,48 @@ class Reader:
         spans = [(a64[0][i], a64[1][i], a64[2][i], a64[3][i], a32[0][i], bool(a32[1][i])) for i in range(ns.value)]
         return spans, nb.value, fb.value
 
+    @staticmethod
+    def _cast_ranges(ranges):
+        import torch
+        codes = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.bfloat16: _lib.DTYPE_BF16}
+        arr = (_lib.CvCastRange * max(1, len(ranges)))()
+        for i, (off, row_len, rows, file_pitch, ptr, dst_pitch, src, dst) in enumerate(ranges):
+            if src == dst:
+                sc = dc = codes.get(src, _lib.DTYPE_NONE)
+            elif src in codes and dst in codes:
+                sc, dc = codes[src], codes[dst]
+            else:
+                raise ValueError("range %d: conversions are between float32, float16 and bfloat16 only, not %s -> %s" % (i, src, dst))
+            a = arr[i]
+            a.file_off, a.row_len, a.rows, a.file_pitch, a.d_dst, a.dst_pitch = off, row_len, rows, file_pitch, ptr, dst_pitch
+            a.src_dtype, a.dst_dtype = sc, dc
+        return arr
+
+    def readv_cast_device(self, ranges, stream: int = 0) -> int:
+        """Cast device read: `ranges` is a list of (file_off, row_len, rows, file_pitch, d_ptr, dst_pitch, src_dtype, dst_dtype) with torch
+        dtypes.  A range with src_dtype == dst_dtype is a range of readv_strided_device; any other converts its elements on the GPU (float32,
+        float16 and bfloat16 into one another, round-to-nearest-even): its file side is in source bytes, d_ptr and dst_pitch in destination
+        bytes.  Every block a converting range touches is verified before it is converted.  -> bytes delivered."""
+        n = ctypes.c_int64()
+        _check(_lib.lib().cv_readv_cast_device(self._h, self._cast_ranges(ranges), len(ranges), ctypes.c_void_p(stream), ctypes.byref(n)))
+        return n.value
+
+    def readv_cast_plan(self, ranges):
+        """What readv_cast_device(ranges) executes (host-only; d_ptr is looked at for its alignment only).  -> (spans, n_blocks, fetch_bytes)
+        as readv_strided_plan."""
+        arr = self._cast_ranges(ranges)
+        ns, nb, fb = ctypes.c_int32(), ctypes.c_int64(), ctypes.c_int64()
+        L = _lib.lib()
+        _check(L.cv_readv_cast_plan(self._h, arr, len(ranges), None, None, None, None, None, None, 0, ctypes.byref(ns), ctypes.byref(nb),
+                                    ctypes.byref(fb)))
+        cap = max(1, ns.value)
+        a64 = [(ctypes.c_int64 * cap)() for _ in range(4)]
+        a32 = [(ctypes.c_int32 * cap)() for _ in range(2)]
+        _check(L.cv_readv_cast_plan(self._h, arr, len(ranges), a64[0], a64[1], a64[2], a64[3], a32[0], a32[1], cap, ctypes.byref(ns),
+                                    ctypes.byref(nb), ctypes.byref(fb)))
+        spans = [(a64[0][i], a64[1][i], a64[2][i], a64[3][i], a32[0][i], bool(a32[1][i])) for i in range(ns.value)]
+        return spans, nb.value, fb.value
+
     def fuse_read_device(self, pos: int, size: int, d_scratch: int, d_page_base: int, page_offsets, page_size: int,
                          stream: int = 0) -> int:
         arr = (ctypes.c_uint64 * len(page_offsets))(*page_offsets)

@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import CvFrameDesc, CvSeg, CvStreamDesc, CvStridedSeg, check
+from ._lib import CvCastSeg, CvFrameDesc, CvSeg, CvStreamDesc, CvStridedSeg, check
 
 POLY_IEEE, POLY_CASTAGNOLI = 0, 1
 
@@ -107,6 +107,22 @@ def strided_segs_to_device(segs, device):
 def gather_strided(src, d_segs, n, total_bytes, dst, stream=None):
     check(_lib.lib().cvk_gather_strided(_ptr(src), _ptr(d_segs), n, total_bytes, _ptr(dst), _stream_ptr(stream)),
           "cvk_gather_strided")
+
+
+def cast_segs_to_device(segs, device):
+    """segs: list of (src_off, dst_off, elems, rows, src_pitch, dst_pitch, src_dtype, dst_dtype) with _lib.DTYPE_* codes; `first` (the
+    work distribution) is filled here.  -> (device table, total elements)"""
+    arr = (CvCastSeg * len(segs))()
+    first = total = 0
+    for i, (so, do, elems, rows, sp, dp, sdt, ddt) in enumerate(segs):
+        arr[i] = CvCastSeg(so, do, elems, rows, sp, dp, first, sdt, ddt)
+        first += rows * _lib.cast_row_chunks(elems)
+        total += elems * rows
+    return _struct_array_to_device(arr, device), total
+
+
+def gather_cast(src, d_segs, n, total_elems, dst, stream=None):
+    check(_lib.lib().cvk_gather_cast(_ptr(src), _ptr(d_segs), n, total_elems, _ptr(dst), _stream_ptr(stream)), "cvk_gather_cast")
 
 
 def deinterleave_blocks(gathered, shard_stride, world, block_size, n_blocks, file_len, dst, stream=None):

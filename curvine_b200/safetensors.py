@@ -113,15 +113,38 @@ def _is_integral(x) -> bool:
     return isinstance(x, numbers.Integral) and not isinstance(x, bool)
 
 
-def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=None) -> List[tuple]:
+def _cast_targets(data_start: int, entries: Dict[str, tuple], selected, dtype) -> Dict[str, object]:
+    """{name: dtype of the result} for load_file(dtype=...): the float32, float16 and bfloat16 tensors become `dtype`, the others stay as
+    stored.  Raises ValueError for a target dtype other than those three, for a selected float tensor of another width (float64, float8:
+    not converted) and for a converting tensor whose data offset is not a multiple of its element size."""
+    import torch
+    floats = (torch.float32, torch.float16, torch.bfloat16)
+    if dtype not in floats:
+        raise ValueError("dtype %s: loads convert to float32, float16 or bfloat16 only" % (dtype,))
+    out = {}
+    for name in selected:
+        stored, _, begin, end = entries[name]
+        if stored.is_floating_point and stored not in floats:
+            raise ValueError("%s: %s tensors are not converted on load (only float32, float16 and bfloat16 are)" % (name, stored))
+        out[name] = dtype if stored in floats else stored
+        if out[name] != stored and (data_start + begin) % stored.itemsize:
+            raise ValueError("%s: data offset %d is not a multiple of its %d-byte element size" % (name, data_start + begin, stored.itemsize))
+    return out
+
+
+def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=None, dtype=None) -> List[tuple]:
     """The loader's ranges, without a GPU.  -> [(name, dtype, shape of the result, range)] for the selected names, in order, where range
     is (file_off, row_len, rows, file_pitch, dst_pitch) of Reader.readv_strided_device (d_ptr left out), or None when the tensor has no
     bytes to read.  An unsliced tensor is one row.  slices[name] = (dim, start, stop) keeps [start, stop) of dimension dim: the rows are
     the prod(shape[:dim]) pieces of the row-major tensor that hold it, each (stop - start) * inner bytes long and shape[dim] * inner bytes
-    apart (inner = prod(shape[dim+1:]) * itemsize), landing back to back.  Raises KeyError for a sliced name the file does not hold,
-    ValueError for a malformed slice or a sliced name outside `selected`."""
+    apart (inner = prod(shape[dim+1:]) * itemsize), landing back to back.  With `dtype` (float32, float16 or bfloat16) the float32,
+    float16 and bfloat16 tensors come back in `dtype`, the others as stored: dtype is the result's and range is (file_off, row_len, rows,
+    file_pitch, dst_pitch, stored dtype, result dtype) of Reader.readv_cast_device, its file side in stored bytes and its dst_pitch in
+    result bytes.  Raises KeyError for a sliced name the file does not hold, ValueError for a malformed slice, a sliced name outside
+    `selected`, or a tensor load_file(dtype=...) cannot convert (see _cast_targets)."""
     slices = dict(slices or {})
     sel = set(selected)
+    targets = _cast_targets(data_start, entries, selected, dtype) if dtype is not None else None
     for name, spec in slices.items():
         if name not in entries:
             raise KeyError("the file holds no tensor named %r" % (name,))
@@ -140,33 +163,39 @@ def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=Non
             raise ValueError("%s: [%d, %d) is not a slice of dimension %d of size %d" % (name, start, stop, dim, shape[d]))
     out = []
     for name in selected:
-        dtype, shape, begin, end = entries[name]
+        stored, shape, begin, end = entries[name]
+        dt = targets[name] if targets is not None else stored
+        tail = (stored, dt) if targets is not None else ()  # the dtypes of a readv_cast_device range
         if name not in slices:
-            out.append((name, dtype, shape, (data_start + begin, end - begin, 1, 0, 0) if end > begin else None))
+            out.append((name, dt, shape, (data_start + begin, end - begin, 1, 0, 0) + tail if end > begin else None))
             continue
         dim, start, stop = (int(x) for x in slices[name])
         d = dim % len(shape)
-        inner = dtype.itemsize
+        inner = 1  # elements
         for x in shape[d + 1:]:
             inner *= x
         rows = 1
         for x in shape[:d]:
             rows *= x
-        row_len = (stop - start) * inner
+        row_len = (stop - start) * inner * stored.itemsize
         res = shape[:d] + (stop - start,) + shape[d + 1:]
-        rng = (data_start + begin + start * inner, row_len, rows, shape[d] * inner, row_len) if row_len and rows else None
-        out.append((name, dtype, res, rng))
+        rng = (data_start + begin + start * inner * stored.itemsize, row_len, rows, shape[d] * inner * stored.itemsize,
+               (stop - start) * inner * dt.itemsize) + tail if row_len and rows else None
+        out.append((name, dt, res, rng))
     return out
 
 
 def load_file(fs: "_fs.CurvineFileSystem", path: str, device=None, names: Optional[Iterable[str]] = None,
-              verify: bool = True, slices: Optional[Dict[str, tuple]] = None) -> Dict[str, "object"]:
+              verify: bool = True, slices: Optional[Dict[str, tuple]] = None, dtype=None) -> Dict[str, "object"]:
     """The tensors of safetensors file `path` (all of them, or those in `names`) as tensors on `device` (default: the current CUDA
     device).  One vectored read moves them: blocks that no selected tensor touches are not fetched, and every touched block is
     CRC-verified whole, including the bytes of unselected neighbours that share it.  `slices` maps a name to (dim, start, stop): that
     tensor comes back contiguous with shape[dim] = stop - start -- a tensor-parallel rank's shard, without the rest of the tensor ever
-    reaching HBM (see plan_ranges).  Raises IOError when a block fails verification and `verify` is set, SafetensorsError for a malformed
-    header, KeyError for a name the file does not hold, ValueError for a malformed slice (all before anything is allocated or read)."""
+    reaching HBM (see plan_ranges).  `dtype` (torch.float32, torch.float16 or torch.bfloat16) converts every float32, float16 and bfloat16
+    tensor to it on the GPU in the same read, bit-identical to Tensor.to() on the CPU; integer and bool tensors come back as stored.  The
+    stored copy never exists in HBM: a converted tensor's blocks pass through the reader's bounded staging.  Raises IOError when a block
+    fails verification and `verify` is set, SafetensorsError for a malformed header, KeyError for a name the file does not hold,
+    ValueError for a malformed slice or a tensor `dtype` cannot convert (all before anything is allocated or read)."""
     import torch
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     r, data_start, entries = _open_header(fs, path)
@@ -175,15 +204,19 @@ def load_file(fs: "_fs.CurvineFileSystem", path: str, device=None, names: Option
         for name in selected:
             if name not in entries:
                 raise KeyError("%s holds no tensor named %r" % (path, name))
-        plan = plan_ranges(data_start, entries, selected, slices)
+        plan = plan_ranges(data_start, entries, selected, slices, dtype)
         out, ranges = {}, []
-        for name, dtype, shape, rng in plan:
-            t = torch.empty(shape, dtype=dtype, device=dev)
+        for name, dt, shape, rng in plan:
+            t = torch.empty(shape, dtype=dt, device=dev)
             out[name] = t
             if rng is not None:
-                file_off, row_len, rows, file_pitch, dst_pitch = rng
-                ranges.append((file_off, row_len, rows, file_pitch, t.data_ptr(), dst_pitch))
-        r.readv_strided_device(ranges, torch.cuda.current_stream(dev).cuda_stream)
+                file_off, row_len, rows, file_pitch, dst_pitch = rng[:5]
+                ranges.append((file_off, row_len, rows, file_pitch, t.data_ptr(), dst_pitch) + tuple(rng[5:]))
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        if dtype is None:
+            r.readv_strided_device(ranges, stream)
+        else:  # one call still: the ranges that convert nothing have src == dst, and their whole blocks land in place
+            r.readv_cast_device(ranges, stream)
         _, bad, _ = r.verify()
         if verify and bad:
             raise IOError("%d blocks of %s failed CRC verification" % (bad, path))

@@ -159,6 +159,30 @@ int64_t cv_readv_strided_device(cv_reader* r, const CvStridedRange* ranges, int3
 int64_t cv_readv_strided_plan(cv_reader* r, const CvStridedRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len,
                               int64_t* rows, int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks,
                               int64_t* fetch_bytes);
+/* Cast device read: cv_readv_strided_device where a range may also convert its elements on the GPU, from src_dtype as stored in the
+ * file to dst_dtype in HBM (CV_DTYPE_F32 / _F16 / _BF16 into one another, rounded as cvk_gather_cast).  src_dtype == dst_dtype
+ * (CV_DTYPE_NONE included) is no conversion: such a range plans and lands exactly as the same CvStridedRange.  The file side of a
+ * converting range (file_off, row_len, file_pitch) is in source bytes, the destination side (d_dst, dst_pitch) in destination bytes:
+ * row k of row_len / src size elements lands at d_dst + k*dst_pitch, row_len / src size * dst size bytes long.  Every block a
+ * converting range touches goes through the device staging (none is direct), so its CRC is checked before a byte of it is converted.
+ * *nbytes = bytes delivered: sum of rows * row_len / src size * dst size.  Errors besides those of cv_readv_strided_device (cv_last_error
+ * names the range): a dtype code other than the four above; a conversion involving CV_DTYPE_NONE; file_off, row_len or (rows > 1)
+ * file_pitch not a multiple of the source element size; d_dst or (rows > 1) dst_pitch not a multiple of the destination element
+ * size; rows > 1 with dst_pitch shorter than a destination row; a file whose block size is not a multiple of the source element size. */
+typedef struct CvCastRange {
+    int64_t file_off;
+    int64_t row_len;    /* source bytes per row */
+    int64_t rows;
+    int64_t file_pitch;
+    void* d_dst;
+    int64_t dst_pitch;  /* destination bytes between row starts */
+    int32_t src_dtype;  /* CV_DTYPE_* */
+    int32_t dst_dtype;
+} CvCastRange;          /* 56 bytes */
+int64_t cv_readv_cast_device(cv_reader* r, const CvCastRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes);
+/* The plan cv_readv_cast_device executes, with the outputs of cv_readv_strided_plan (block_off and len in source bytes). */
+int64_t cv_readv_cast_plan(cv_reader* r, const CvCastRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len, int64_t* rows,
+                           int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes);
 /* FUSE-shaped device read: seek(pos), read len bytes into HBM scratch, then scatter them into n_pages page
  * buffers (d_page_base + page_offsets[i], page_size each; last one partial) with the K3 gather kernel. */
 int64_t cv_fuse_read_device(cv_reader* r, int64_t pos, int64_t len, void* d_scratch, void* d_page_base,

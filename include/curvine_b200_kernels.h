@@ -17,6 +17,7 @@
  *   cvk_gather_pages    Reader::fuse_read + as_iovec/writev curvine-common/src/fs/reader.rs:101-124,
  *                                                           curvine-fuse/src/session/fuse_response.rs:49-60,171-175
  *   cvk_gather_strided  (no reference counterpart: the rows of tensor-parallel slices of a checkpoint, strided reads)
+ *   cvk_gather_cast     (no reference counterpart: checkpoint tensors converted to another float type on load)
  *   cvk_pack_frames     RpcMessage::encode_protocol +      orpc/src/message/rpc_message.rs:301-311,
  *                       RpcFrame::send/write_region          orpc/src/handler/rpc_frame.rs:97-121,205-220
  *                       (worker ReadHandler::read response)  curvine-server/src/worker/handler/read_handler.rs:143-183
@@ -109,6 +110,31 @@ typedef struct CvStridedSeg {
     uint64_t dst_pitch;
 } CvStridedSeg;
 
+/* element types of cvk_gather_cast and of cast reads (CvCastRange).  CV_DTYPE_NONE: bytes as stored, no conversion. */
+#define CV_DTYPE_NONE 0
+#define CV_DTYPE_F32 1
+#define CV_DTYPE_F16 2
+#define CV_DTYPE_BF16 3
+
+/* Work chunks of one row of `elems` elements in cvk_gather_cast: a chunk is 8 elements whose destination starts 16-byte aligned, plus
+ * a head chunk for the elements in front of the first aligned one. */
+#define CV_CAST_ROW_CHUNKS(elems) ((elems) ? ((uint64_t)(elems) + 14) / 8 : 0)
+
+/* cast segment: rows equally spaced rows of elems elements, converted from src_dtype to dst_dtype,
+ * d_dst[dst_off + k*dst_pitch ..) = convert(d_src[src_off + k*src_pitch ..)) for k < rows (offsets and pitches in bytes).
+ * `first` is the work distribution, filled by the host: the exclusive prefix over the table of rows * CV_CAST_ROW_CHUNKS(elems). */
+typedef struct CvCastSeg {
+    uint64_t src_off;
+    uint64_t dst_off;
+    uint64_t elems;      /* elements per row */
+    uint64_t rows;
+    uint64_t src_pitch;
+    uint64_t dst_pitch;
+    uint64_t first;      /* first work chunk of this segment */
+    int32_t src_dtype;   /* CV_DTYPE_F32 / _F16 / _BF16 */
+    int32_t dst_dtype;
+} CvCastSeg;             /* 64 bytes */
+
 /* Build the per-device constant tables (both polynomials).  Optional: every launcher does it lazily. */
 int cvk_init(int device);
 
@@ -149,6 +175,16 @@ int cvk_gather_pages(const uint8_t* d_src, const CvSeg* d_segs, uint32_t n, uint
  * total_bytes = sum of len * rows.  Algorithmic bytes: reads N, writes N. */
 int cvk_gather_strided(const uint8_t* d_src, const CvStridedSeg* d_segs, uint32_t n, uint64_t total_bytes, uint8_t* d_dst,
                        cv_stream_t stream);
+
+/* K5: gather with a dtype conversion, every row of every segment: F32, F16 and BF16 into one another, IEEE round-to-nearest-even
+ * (subnormals, signed zeros, infinities; F32 -> F16 overflows to inf), bit-identical to torch's CPU Tensor.to() for every non-NaN input;
+ * a NaN stays a NaN (its payload may differ).  F16 <-> BF16 goes through F32, which is exact: one rounding.  A segment with
+ * src_dtype == dst_dtype is a copy; one with a code other than the three is skipped.  Sources and destinations need only their
+ * element alignment; a row is converted in chunks of 8 elements whose destination is 16-byte aligned (a scalar head and tail around
+ * them), the chunks of all segments spread over all SMs, and the launcher neither reads the table back nor synchronises.
+ * total_elems = sum of elems * rows (sizes the grid; 0 launches nothing).  Rows of different segments must not overlap in d_dst.
+ * Algorithmic bytes: reads N * src size, writes N * dst size. */
+int cvk_gather_cast(const uint8_t* d_src, const CvCastSeg* d_segs, uint32_t n, uint64_t total_elems, uint8_t* d_dst, cv_stream_t stream);
 
 /* K4: worker-side inverse of K2.  For frame f: write the 22-byte prefix (+ no header) at
  * d_wire + d_desc[f].wire_off, copy d_src[dst_off .. +data_len) behind it, and CRC the source bytes
