@@ -368,9 +368,6 @@ __global__ void __launch_bounds__(1024) scan_tiles_kernel(const uint32_t* __rest
 constexpr uint32_t kTmWords = 4 * 256 * 32;  // replicated x^4096 tables: [table][byte][lane]
 constexpr uint32_t kSmemWords = kTmWords + 256 + 64 + 16;
 constexpr uint32_t kSmemBytes = kSmemWords * 4;
-constexpr int kStageCrc = 6;    // row slots per warp of the staged CRC+copy walk (tables 129 KB + 32 x 6 x 512 B = 225 KB of 227)
-constexpr int kStageCopy = 12;  // ... of the staged copy-only walk (32 x 12 x 512 B = 192 KB)
-static_assert(kSmemBytes % 16 == 0, "stage slots must be 16-byte aligned");
 
 __device__ __forceinline__ uint4 ld_stream(const uint4* p) {
     uint4 r;
@@ -550,75 +547,11 @@ __device__ __forceinline__ void walk_aligned_copy(const uint8_t* src, uint8_t* d
     c.a0 = a0, c.a1 = a1, c.a2 = a2, c.a3 = a3;
 }
 
-// ---- shared-memory staged DST walk (cp.async): rows in flight live in shared memory, not in registers.
-// Every warp owns S row slots of 512 bytes.  Lane l copies its aligned source vector of row r into slot r % S with a
-// 16-byte cp.async (L2 only), one commit group per row; the consumer side waits until rows j and j+1 have landed
-// (wait_group S-2), reads its own vector and its right neighbour's (lane 31: lane 0 of the following row) back with two
-// LDS.128, funnel-shifts the 16 output bytes together, stores them and feeds the CRC chains, then refills the slot with
-// row j+S.  A warp so keeps S-1 rows (CRC+copy: 5 x 512 B, copy-only: 11 x 512 B) in flight all the time, independent of
-// the 64-register budget of the 1024-thread CTA.
-__device__ __forceinline__ void cp_async16(uint32_t smem_addr, const void* gptr) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_addr), "l"(gptr) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-    uint4 r;
-    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr) : "memory");
-    return r;
-}
-
-template <bool CRC, int Q, int S>
-__device__ __forceinline__ void walk_staged(const uint8_t* src, uint8_t* dst, uint32_t L, uint32_t lane, uint32_t tl, Chains& c,
-                                            uint32_t stage) {
-    if (L == 0) return;
-    const uint32_t sh = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(src) & 15u);
-    const uint4* bp = reinterpret_cast<const uint4*>(src - sh) + lane;
-    uint4* dp = reinterpret_cast<uint4*>(dst) + lane;
-    const uint32_t R = L >> 9, nv = (L & 511u) >> 4;
-    const uint32_t nvec = (L >> 4) + (sh ? 1u : 0u);  // aligned vectors that hold the L bytes
-    const uint32_t rows = R + (nv ? 1u : 0u);
-    const uint32_t r8 = (sh & 3u) * 8u;
-    const uint32_t mine = stage + lane * 16u;
-    const uint32_t right = stage + ((lane + 1u) & 31u) * 16u;
-    uint32_t a0 = c.a0, a1 = c.a1, a2 = c.a2, a3 = c.a3;
-#pragma unroll
-    for (int r = 0; r < S; r++) {
-        if (r * 32u + lane < nvec) cp_async16(mine + r * 512u, bp + r * 32);
-        cp_async_commit();
-    }
-    uint32_t slot = 0;  // slot of row j
-    for (uint32_t j = 0; j < rows; j++) {
-        cp_async_wait<S - 2>();  // groups 0 .. j+1 done: rows j and j+1 are in shared memory (this lane's part)
-        __syncwarp();            // ... and every other lane's
-        const uint32_t nslot = slot + 1 == S ? 0u : slot + 1;
-        const uint4 ra = lds128(mine + slot * 512u);
-        const uint4 nb = lds128(right + (lane == 31 ? nslot : slot) * 512u);
-        const uint4 v = shift_window<Q>(ra, nb, r8);
-        if (j < R) {
-            st_vec(dp + j * 32, v);
-            if (CRC) CV_STEP(v);
-        } else if (lane < nv) {
-            st_vec(dp + j * 32, v);
-            c.vr = v;
-        }
-        __syncwarp();  // all lanes are done with slot `slot` before it is refilled
-        const uint32_t nr = j + S;
-        if (nr * 32u + lane < nvec) cp_async16(mine + slot * 512u, bp + nr * 32);
-        cp_async_commit();
-        slot = nslot;
-    }
-    c.a0 = a0, c.a1 = a1, c.a2 = a2, c.a3 = a3;
-}
-
 // One warp walks L bytes (multiple of 16) starting at src (dst is 16-byte aligned when DST; src is 16-byte
 // aligned when !DST).  Returns the segment's raw CRC in every lane (0 when !CRC).  T = rows per tile of the DST walks.
-template <bool CRC, bool DST, int T, int S>
+template <bool CRC, bool DST, int T>
 __device__ __forceinline__ uint32_t walk_segment(const uint8_t* src, uint8_t* dst, uint32_t L, uint32_t lane,
-                                                 const uint32_t* smem, uint32_t poly, uint32_t stage) {
+                                                 const uint32_t* smem, uint32_t poly) {
     const uint32_t tl = static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + lane * 4u;
     const uint32_t* t0 = smem + kTmWords;
     const uint32_t* xp128 = t0 + 256;
@@ -650,14 +583,7 @@ __device__ __forceinline__ uint32_t walk_segment(const uint8_t* src, uint8_t* ds
         c.a0 = a0, c.a1 = a1, c.a2 = a2, c.a3 = a3;
     } else {
         const uint32_t sh = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(src) & 15u);
-        if (S > 0) {
-            switch (sh >> 2) {  // warp-uniform; sh == 0 runs as Q = 0 with a zero bit shift
-                case 0: walk_staged<CRC, 0, S ? S : 2>(src, dst, L, lane, tl, c, stage); break;
-                case 1: walk_staged<CRC, 1, S ? S : 2>(src, dst, L, lane, tl, c, stage); break;
-                case 2: walk_staged<CRC, 2, S ? S : 2>(src, dst, L, lane, tl, c, stage); break;
-                default: walk_staged<CRC, 3, S ? S : 2>(src, dst, L, lane, tl, c, stage); break;
-            }
-        } else if (sh == 0) {
+        if (sh == 0) {
             walk_aligned_copy<CRC, T>(src, dst, L, lane, tl, c);
         } else {
             switch (sh >> 2) {  // warp-uniform
@@ -734,7 +660,7 @@ __device__ __forceinline__ Unit ld_unit(const Unit* p) {
     return un;
 }
 
-template <bool CRC, bool DST, int T, int S = 0>
+template <bool CRC, bool DST, int T>
 __global__ void __launch_bounds__(1024, 1)
     walk_kernel(const Unit* __restrict__ units, const uint32_t* __restrict__ total_units, const CrcConsts* __restrict__ cc,
                 uint32_t* __restrict__ partial, uint32_t partial_cap, uint32_t* __restrict__ headraw, uint32_t* __restrict__ tailraw) {
@@ -756,12 +682,10 @@ __global__ void __launch_bounds__(1024, 1)
     }
     const uint32_t* t0 = smem + kTmWords;
     if (u0 + warp >= u1) return;
-    // staged walks: this warp's S row slots sit behind the tables (CRC) or at the start of shared memory (copy-only)
-    const uint32_t stage = static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + (CRC ? kSmemBytes : 0u) + warp * (S * 512u);
     Unit cur = ld_unit(units + u0 + warp);
     for (uint32_t u = u0 + warp; u < u1; u += 32) {
         const Unit nxt = ld_unit(units + (u + 32 < u1 ? u + 32 : u));  // next unit's record travels behind this walk
-        const uint32_t raw = walk_segment<CRC, DST, T, S>(cur.src, cur.dst, cur.L, lane, smem, poly, stage);
+        const uint32_t raw = walk_segment<CRC, DST, T>(cur.src, cur.dst, cur.L, lane, smem, poly);
         if (CRC && lane == 0) partial[u] = raw;
         if (cur.head && lane == 1) {
             const uint32_t r = walk_bytes<CRC, DST>(cur.src - cur.head, DST ? cur.dst - cur.head : nullptr, cur.head, t0);
@@ -1063,10 +987,6 @@ __global__ void __launch_bounds__(256) gather_cast_kernel(const uint8_t* __restr
 // ------------------------------------------------------------------ host side
 
 static std::atomic<uint64_t> g_launches{0};
-// Tuning of the DST walkers (cvk_tune; defaults chosen from tools/kbench.py sweeps): rows per tile, and
-// register-tiled vs shared-memory staged walks.  (An L1::no_allocate load flavour was swept too: no gain, removed.)
-static std::atomic<int> g_tile_crc_dst{4}, g_tile_copy{2};
-static std::atomic<bool> g_staged{false};  // cvk_tune(3, 1) / CVK_STAGED=1: shared-memory staged (cp.async) DST walks for local sources
 static std::mutex g_mu;
 constexpr int kMaxDev = 16;
 static CrcConsts* g_consts[kMaxDev][2];
@@ -1130,11 +1050,7 @@ static int ensure_device(int* dev_out) {
         CV_TRY(cudaMemPoolSetAttribute(g_pool[dev], cudaMemPoolAttrReleaseThreshold, &keep));
     }
     CV_TRY(cudaFuncSetAttribute(walk_kernel<true, false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    CV_TRY(cudaFuncSetAttribute(walk_kernel<true, true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     CV_TRY(cudaFuncSetAttribute(walk_kernel<true, true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    CV_TRY(cudaFuncSetAttribute(walk_kernel<true, true, 4, kStageCrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes + kStageCrc * 512 * 32));
-    CV_TRY(cudaFuncSetAttribute(walk_kernel<false, true, 2, kStageCopy>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageCopy * 512 * 32));
-    if (const char* e = getenv("CVK_STAGED")) g_staged.store(atoi(e) != 0);
     g_ready[dev] = true;
     return 0;
 }
@@ -1236,27 +1152,16 @@ static void launch_expand(const Workspace& w, uint32_t n, uint32_t seg_shift, cu
     expand_units_kernel<DST><<<cdiv(w.partial_cap, 256), 256, 0, st>>>(w.pieces, n, w.prefix, seg_shift, w.units, w.partial_cap);
 }
 
+// Rows per tile of the DST walks: 4 for CRC+copy, 2 for copy-only (tools/kbench.py, DESIGN §3).
 static void launch_walk_crc_dst(int dev, cudaStream_t st, const Workspace& w, uint32_t n, const CrcConsts* cc) {
-    const dim3 grid(g_sm_count[dev]), block(1024);
-    if (g_staged.load(std::memory_order_relaxed)) {
-        walk_kernel<true, true, 4, kStageCrc><<<grid, block, kSmemBytes + kStageCrc * 512 * 32, st>>>(CV_WALK_ARGS);
-    } else {  // the register-tiled walks differ only in rows per tile: one launch of the chosen instance
-        auto walk = g_tile_crc_dst.load(std::memory_order_relaxed) == 2 ? walk_kernel<true, true, 2> : walk_kernel<true, true, 4>;
-        walk<<<grid, block, kSmemBytes, st>>>(CV_WALK_ARGS);
-    }
+    walk_kernel<true, true, 4><<<g_sm_count[dev], 1024, kSmemBytes, st>>>(CV_WALK_ARGS);
 }
 
 // copy-only walk: no shared memory, one CTA per SM (the kernels need > 32 registers, so two 1024-thread CTAs never fit).
-// peer = some source may be another GPU's HBM mapped over NVLink: register-tiled walk with plain coherent loads only.
-static void launch_walk_copy(int dev, cudaStream_t st, const Workspace& w, uint32_t n, bool peer = false) {
-    const dim3 grid(g_sm_count[dev]), block(1024);
+// Sources may be another GPU's HBM mapped over NVLink (cvk_gather_shards_p2p): the DST walks use plain coherent loads only.
+static void launch_walk_copy(int dev, cudaStream_t st, const Workspace& w, uint32_t n) {
     const CrcConsts* cc = nullptr;
-    if (!peer && g_staged.load(std::memory_order_relaxed))
-        walk_kernel<false, true, 2, kStageCopy><<<grid, block, kStageCopy * 512 * 32, st>>>(CV_WALK_ARGS);
-    else if (g_tile_copy.load(std::memory_order_relaxed) == 4)
-        walk_kernel<false, true, 4><<<grid, block, 0, st>>>(CV_WALK_ARGS);
-    else
-        walk_kernel<false, true, 2><<<grid, block, 0, st>>>(CV_WALK_ARGS);
+    walk_kernel<false, true, 2><<<g_sm_count[dev], 1024, 0, st>>>(CV_WALK_ARGS);
 }
 #undef CV_WALK_ARGS
 static inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_relaxed); }
@@ -1278,10 +1183,7 @@ int cvk_init(int device) {
 }
 
 int cvk_tune(int what, int value) {
-    if (what == 0 && (value == 2 || value == 4)) g_tile_crc_dst.store(value);
-    else if (what == 1 && (value == 2 || value == 4)) g_tile_copy.store(value);
-    else if (what == 3 && (value == 0 || value == 1)) g_staged.store(value != 0);
-    else if (what == 4 && (value == 0 || (value >= 12 && value <= 20))) g_seg_shift_override.store(value);
+    if (what == 4 && (value == 0 || (value >= 12 && value <= 20))) g_seg_shift_override.store(value);
     else if (what == 5 && (value == 0 || value == 1)) g_small_path.store(value != 0);
     else if (what == 6 && value >= 0 && value <= int(kStridedTrainRows)) g_strided_train.store(value ? uint32_t(value) : kStridedTrainRows);
     else return int(cudaErrorInvalidValue);
@@ -1425,10 +1327,10 @@ int cvk_pack_frames(const uint8_t* d_src, const CvFrameDesc* d_desc, uint32_t n_
                          stream);
 }
 
-static int copy_pieces(Workspace& w, uint32_t n, uint32_t seg_shift, int dev, cudaStream_t st, bool peer = false) {
+static int copy_pieces(Workspace& w, uint32_t n, uint32_t seg_shift, int dev, cudaStream_t st) {
     const int n_scan = launch_scan(w, n, st);
     launch_expand<true>(w, n, seg_shift, st);
-    launch_walk_copy(dev, st, w, n, peer);
+    launch_walk_copy(dev, st, w, n);
     count_launch(2 + n_scan);
     return ws_finish(w, st);
 }
@@ -1554,7 +1456,7 @@ int cvk_gather_shards_p2p(const uint8_t* const* shard_ptrs, uint32_t world, uint
     }
     prep_gather_shards_kernel<<<cdiv(n, 256), 256, 0, st>>>(d_ptrs, world, block_size, n_blocks, file_len, d_dst, seg_shift, w.pieces, w.counts);
     count_launch();
-    return copy_pieces(w, n, seg_shift, dev, st, true);
+    return copy_pieces(w, n, seg_shift, dev, st);
 }
 
 }  // extern "C"

@@ -213,13 +213,11 @@ int cvk_gather_shards_p2p(const uint8_t* const* shard_ptrs, uint32_t world, uint
 int cvk_profile_enable(int on);
 int cvk_profile_collect(double* walk_ms_total, uint32_t* walk_launches);
 
-/* Tuning hook for the DST row walkers.  what 0: rows per tile (= 512-byte rows a warp keeps in flight in registers) of
- * the CRC+copy walkers (K2/K4), value in {2,4}; what 1: of the copy-only walker (K3/deinterleave/P2P gather), value in
- * {2,4}; what 3: shared-memory staged (cp.async) DST walks (1) or register-tiled ones (0, default; CVK_STAGED=1 in the
- * environment flips the default); what 4: segment size 2^value bytes
- * (12..20) for every launcher instead of the size-derived choice, 0 = back to automatic; what 5: 0 routes inputs of at most ~1 MiB through the general launch train
- * instead of the single-launch small-input kernels (default 1); what 6: rows per train of cvk_gather_strided, 1..2^22, 0 = back to
- * the default 2^22.  Process-wide; results are identical for every setting (tools/kbench.py sweeps it). */
+/* Tuning hook: forces the other side of launch choices the library otherwise makes from the input.  what 4: segment size
+ * 2^value bytes (12..20) for every launcher instead of the size-derived choice, 0 = back to automatic; what 5: 0 routes inputs
+ * of at most ~1 MiB through the general launch train instead of the single-launch small-input kernels (default 1); what 6: rows
+ * per train of cvk_gather_strided, 1..2^22, 0 = back to the default 2^22.  Any other what, or a value out of range, returns
+ * cudaErrorInvalidValue.  Process-wide; results are identical for every setting. */
 int cvk_tune(int what, int value);
 
 /* Number of kernel launches issued by this library in this process (bench.py's gpu_launches claim). */

@@ -73,14 +73,15 @@ assert not bad, bad
     assert r.returncode == 0 and "survived []" in r.stdout, (r.returncode, r.stdout[-1500:])
 
 
-def test_tuning_hook_validates_its_arguments_without_a_gpu():
-    """cvk_tune only flips process-wide launch choices: legal values are accepted, everything else is cudaErrorInvalidValue (1)."""
+def test_tuning_hook_takes_only_segment_small_path_and_train_settings():
+    """cvk_tune only flips process-wide launch choices the library otherwise makes from the input (what 4, 5, 6): legal values are
+    accepted without a GPU, everything else -- the walker tile and staged-walk settings 0, 1 and 3 included -- is cudaErrorInvalidValue (1)."""
     L = _lib.lib()
-    for what, value in ((0, 2), (0, 4), (1, 4), (1, 2), (3, 1), (3, 0)):
+    for what, value in ((4, 12), (4, 20), (4, 0), (5, 0), (5, 1), (6, 7), (6, 1 << 22), (6, 0)):
         assert L.cvk_tune(what, value) == 0
-    for what, value in ((0, 3), (1, 8), (2, 1), (3, 2), (9, 0)):
+    for what, value in ((0, 3), (1, 8), (2, 1), (3, 2), (9, 0), (0, 4), (1, 2), (3, 0), (4, 11), (4, 21), (5, 2), (6, -1), (6, (1 << 22) + 1)):
         assert L.cvk_tune(what, value) == 1
-    assert L.cvk_tune(0, 4) == 0 and L.cvk_tune(1, 2) == 0 and L.cvk_tune(3, 0) == 0  # back to the defaults
+    assert L.cvk_tune(4, 0) == 0 and L.cvk_tune(5, 1) == 0 and L.cvk_tune(6, 0) == 0  # back to the defaults
 
 
 def test_host_crc_and_generator_match_oracle():

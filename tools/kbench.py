@@ -45,23 +45,13 @@ def main():
     ap.add_argument("--block", type=int, default=4 << 20)
     ap.add_argument("--only", default="")
     ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--tile-crc", type=int, default=0, help="cvk_tune(0, v): rows per tile of the CRC+copy walkers (1, 2, 4)")
-    ap.add_argument("--tile-copy", type=int, default=0, help="cvk_tune(1, v): rows per tile of the copy-only walker (2, 4)")
-    ap.add_argument("--staged", type=int, default=-1, help="cvk_tune(3, v): 1 = shared-memory staged (cp.async) DST walks")
     ap.add_argument("--seg-shift", type=int, default=0, help="cvk_tune(4, v): segment size 2^v bytes for every launcher (0 = automatic)")
     ap.add_argument("--warm-sec", type=float, default=0.25, help="seconds of back-to-back warm-up launches before timing (0 under ncu)")
-    ap.add_argument("--sweep", action="store_true", help="run the K2/K4 and K3 sections once per tile setting, in this process")
     a = ap.parse_args()
     global WARM_SEC
     WARM_SEC = a.warm_sec
     dev = torch.device("cuda:0")
     _lib.check(_lib.lib().cvk_init(0))
-    if a.tile_crc:
-        _lib.check(_lib.lib().cvk_tune(0, a.tile_crc))
-    if a.tile_copy:
-        _lib.check(_lib.lib().cvk_tune(1, a.tile_copy))
-    if a.staged >= 0:
-        _lib.check(_lib.lib().cvk_tune(3, a.staged))
     if a.seg_shift:
         _lib.check(_lib.lib().cvk_tune(4, a.seg_shift))
     total = int(a.gib * (1 << 30)) // a.block * a.block
@@ -78,19 +68,7 @@ def main():
         # one block at a time (latency of a single 4 MiB verify)
         best, med = timeit(lambda: K.crc_blocks_raw(data.data_ptr(), offs, lens, 1, 0, a.block, out), a.iters)
         res["k1_single_block"] = {"us": best * 1e3, "GBps": a.block / best / 1e6}
-    # (rows per tile, no_allocate loads, staged); staged ignores the other two
-    crc_tiles = ((4, 0, 0), (2, 0, 0), (4, 0, 1)) if a.sweep else ((a.tile_crc, None, None),)
-    copy_tiles = ((2, 0, 0), (4, 0, 0), (2, 0, 1)) if a.sweep else ((a.tile_copy, None, None),)
-
-    def tune(which, tc, na, stg):
-        if tc:
-            _lib.check(_lib.lib().cvk_tune(which, tc))
-        if stg is not None:
-            _lib.check(_lib.lib().cvk_tune(3, stg))
-        return ("_staged" if stg else "_T%d_na%d" % (tc, na)) if a.sweep else ""
-
-    for tc, na, stg in (crc_tiles if (not a.only or "k2" in a.only) else ()):
-        sfx = tune(0, tc, na, stg)
+    if not a.only or "k2" in a.only:
         for chunk in (131072, 1 << 20, 4 << 20):
             fpb = a.block // chunk
             stride = a.block + 22 * fpb
@@ -119,7 +97,7 @@ def main():
             ok = bool((err == 0).all().item()) and torch.equal(dst, data[:n])
             K.crc_blocks_raw(data.data_ptr(), offs, lens, nb2, 0, n, out)
             ok = ok and torch.equal(out[:nb2], crc)
-            res["k2_unpack_chunk%d%s" % (chunk, sfx)] = {"payload_GBps": n / best / 1e6, "algo_GBps": (2 * n + 22 * nf) / best / 1e6,
+            res["k2_unpack_chunk%d" % chunk] = {"payload_GBps": n / best / 1e6, "algo_GBps": (2 * n + 22 * nf) / best / 1e6,
                                                 "algo_GBps_med": (2 * n + 22 * nf) / med / 1e6, "ms": best, "ok": ok}
             # K4: the worker-side inverse (pack + CRC at source) over the same frames
             wire2 = torch.empty_like(wire)
@@ -131,12 +109,11 @@ def main():
                                              ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
             best4, med4 = timeit(run4, a.iters)
             ok4 = torch.equal(wire2[:nb2 * stride], wire[:nb2 * stride]) and torch.equal(crc4, crc)
-            res["k4_pack_chunk%d%s" % (chunk, sfx)] = {"payload_GBps": n / best4 / 1e6, "algo_GBps": (2 * n + 22 * nf) / best4 / 1e6,
+            res["k4_pack_chunk%d" % chunk] = {"payload_GBps": n / best4 / 1e6, "algo_GBps": (2 * n + 22 * nf) / best4 / 1e6,
                                               "algo_GBps_med": (2 * n + 22 * nf) / med4 / 1e6, "ms": best4, "ok": ok4}
             del wire2
             del wire, dst
-    for tc, na, stg in (copy_tiles if (not a.only or "k3" in a.only) else ()):
-        sfx = tune(1, tc, na, stg)
+    if not a.only or "k3" in a.only:
         n = total // 2
         page = 131072
         segs = [(i * page + 6, i * page, page) for i in range(n // page - 1)]
@@ -145,22 +122,21 @@ def main():
         tb = sum(s[2] for s in segs)
         best, med = timeit(lambda: K.gather_pages(data, d_segs, len(segs), tb, dst), a.iters)
         ok3 = all(torch.equal(dst[d:d + ln], data[s0:s0 + ln]) for s0, d, ln in (segs[0], segs[len(segs) // 2], segs[-1]))
-        res["k3_gather_128k_misaligned" + sfx] = {"payload_GBps": tb / best / 1e6, "algo_GBps": 2 * tb / best / 1e6, "algo_GBps_med": 2 * tb / med / 1e6, "ms": best, "ok": ok3}
+        res["k3_gather_128k_misaligned"] = {"payload_GBps": tb / best / 1e6, "algo_GBps": 2 * tb / best / 1e6, "algo_GBps_med": 2 * tb / med / 1e6, "ms": best, "ok": ok3}
         segs4k = [(i * 4096 + 4096 + 3, i * 4096, 4096) for i in range(min(n // 4096 - 2, 1 << 18))]
         d_segs4k = K.segs_to_device(segs4k, dev)
         tb4 = sum(s[2] for s in segs4k)
         best, med = timeit(lambda: K.gather_pages(data, d_segs4k, len(segs4k), tb4, dst), a.iters)
-        res["k3_gather_4k_pages_misaligned" + sfx] = {"payload_GBps": tb4 / best / 1e6, "algo_GBps": 2 * tb4 / best / 1e6, "algo_GBps_med": 2 * tb4 / med / 1e6, "ms": best}
+        res["k3_gather_4k_pages_misaligned"] = {"payload_GBps": tb4 / best / 1e6, "algo_GBps": 2 * tb4 / best / 1e6, "algo_GBps_med": 2 * tb4 / med / 1e6, "ms": best}
         segsa = [(i * page + 4096, i * page, page) for i in range(n // page - 1)]
         d_segsa = K.segs_to_device(segsa, dev)
         best, med = timeit(lambda: K.gather_pages(data, d_segsa, len(segsa), tb, dst), a.iters)
-        res["k3_gather_128k_aligned" + sfx] = {"payload_GBps": tb / best / 1e6, "algo_GBps": 2 * tb / best / 1e6, "algo_GBps_med": 2 * tb / med / 1e6, "ms": best}
-        if "torch_copy" not in res:
-            d2 = torch.empty(n, dtype=torch.uint8, device=dev)
-            best, med = timeit(lambda: d2.copy_(data[:n]), a.iters)
-            res["torch_copy"] = {"algo_GBps": 2 * n / best / 1e6, "algo_GBps_med": 2 * n / med / 1e6}
-            del d2
-    res["tile_crc"], res["tile_copy"], res["seg_shift"] = a.tile_crc or "default", a.tile_copy or "default", a.seg_shift or "auto"
+        res["k3_gather_128k_aligned"] = {"payload_GBps": tb / best / 1e6, "algo_GBps": 2 * tb / best / 1e6, "algo_GBps_med": 2 * tb / med / 1e6, "ms": best}
+        d2 = torch.empty(n, dtype=torch.uint8, device=dev)
+        best, med = timeit(lambda: d2.copy_(data[:n]), a.iters)
+        res["torch_copy"] = {"algo_GBps": 2 * n / best / 1e6, "algo_GBps_med": 2 * n / med / 1e6}
+        del d2
+    res["seg_shift"] = a.seg_shift or "auto"
     res["launches"] = K.launch_count()
     print(json.dumps(res, indent=1))
 
