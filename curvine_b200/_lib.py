@@ -53,8 +53,20 @@ class CvCastSeg(ctypes.Structure):
                 ("dst_dtype", ctypes.c_int32)]
 
 
-# include/curvine_b200_kernels.h: element types of cast reads and cvk_gather_cast
-DTYPE_NONE, DTYPE_F32, DTYPE_F16, DTYPE_BF16 = 0, 1, 2, 3
+class CvScaleSeg(ctypes.Structure):
+    _fields_ = [("scale", ctypes.c_void_p), ("block_rows", ctypes.c_uint64), ("block_cols", ctypes.c_uint64), ("scale_cols", ctypes.c_uint64),
+                ("cols", ctypes.c_uint64), ("view0", ctypes.c_uint64), ("view_step", ctypes.c_uint64), ("scale_dtype", ctypes.c_int32),
+                ("pad", ctypes.c_int32)]
+
+
+class CvScaledRange(ctypes.Structure):
+    _fields_ = [("cast", CvCastRange), ("d_scale", ctypes.c_void_p), ("scale_dtype", ctypes.c_int32), ("pad", ctypes.c_int32),
+                ("scale_rows", ctypes.c_int64), ("scale_cols", ctypes.c_int64), ("block_rows", ctypes.c_int64), ("block_cols", ctypes.c_int64),
+                ("cols", ctypes.c_int64), ("first_elem", ctypes.c_int64)]
+
+
+# include/curvine_b200_kernels.h: element types of cast reads and cvk_gather_cast (the two FP8 codes: sources only)
+DTYPE_NONE, DTYPE_F32, DTYPE_F16, DTYPE_BF16, DTYPE_F8_E4M3, DTYPE_F8_E5M2 = 0, 1, 2, 3, 4, 5
 
 
 def cast_row_chunks(elems: int) -> int:
@@ -64,6 +76,7 @@ def cast_row_chunks(elems: int) -> int:
 
 assert ctypes.sizeof(CvStridedRange) == 48 and ctypes.sizeof(CvStridedSeg) == 48
 assert ctypes.sizeof(CvCastRange) == 56 and ctypes.sizeof(CvCastSeg) == 64
+assert ctypes.sizeof(CvScaledRange) == 120 and ctypes.sizeof(CvScaleSeg) == 64
 assert ctypes.sizeof(CvFrameDesc) == 48 and ctypes.sizeof(CvStreamDesc) == 56 and ctypes.sizeof(CvSeg) == 24 and ctypes.sizeof(CvRange) == 24
 
 
@@ -108,6 +121,7 @@ def _declare(L):
     L.cvk_gather_pages.argtypes, L.cvk_gather_pages.restype = [u8p, vp, u32, u64, u8p, vp], i
     L.cvk_gather_strided.argtypes, L.cvk_gather_strided.restype = [u8p, vp, u32, u64, u8p, vp], i
     L.cvk_gather_cast.argtypes, L.cvk_gather_cast.restype = [u8p, vp, u32, u64, u8p, vp], i
+    L.cvk_gather_cast_scaled.argtypes, L.cvk_gather_cast_scaled.restype = [u8p, vp, vp, u32, u64, u8p, vp], i
     L.cvk_pack_frames.argtypes, L.cvk_pack_frames.restype = [u8p, vp, u32, u32, u8p, i, u64, vp, vp], i
     L.cvk_deinterleave_blocks.argtypes = [u8p, u64, u32, u64, u64, u64, u8p, vp]
     L.cvk_deinterleave_blocks.restype = i
@@ -156,6 +170,7 @@ def _declare(L):
                                         cp(i64)]
     L.cv_readv_strided_plan.restype = i64
     L.cv_readv_cast_device.argtypes, L.cv_readv_cast_device.restype = [vp, cp(CvCastRange), i32, vp, cp(i64)], i64
+    L.cv_readv_scaled_device.argtypes, L.cv_readv_scaled_device.restype = [vp, cp(CvScaledRange), i32, vp, cp(i64)], i64
     L.cv_readv_cast_plan.argtypes = [vp, cp(CvCastRange), i32, cp(i64), cp(i64), cp(i64), cp(i64), cp(i32), cp(i32), i32, cp(i32), cp(i64), cp(i64)]
     L.cv_readv_cast_plan.restype = i64
     L.cv_fuse_read_device.argtypes = [vp, i64, i64, vp, vp, vp, i32, i64, vp, cp(i64)]
@@ -192,10 +207,10 @@ class CvReadStats(ctypes.Structure):
 
 # every symbol include/*.h declares (tests check the .so exports all of them)
 EXPORTS = ["cvk_init", "cvk_crc_blocks", "cvk_verify_crcs", "cvk_verify_crcs_masked", "cvk_unpack_frames", "cvk_expand_streams", "cvk_gather_pages",
-           "cvk_gather_strided", "cvk_gather_cast", "cvk_pack_frames", "cvk_deinterleave_blocks", "cvk_gather_shards_p2p", "cvk_launch_count", "cvk_tune", "cvk_profile_enable", "cvk_profile_collect", "cv_last_error", "cv_free", "cv_fs_new",
+           "cvk_gather_strided", "cvk_gather_cast", "cvk_gather_cast_scaled", "cvk_pack_frames", "cvk_deinterleave_blocks", "cvk_gather_shards_p2p", "cvk_launch_count", "cvk_tune", "cvk_profile_enable", "cvk_profile_collect", "cv_last_error", "cv_free", "cv_fs_new",
            "cv_fs_new_from_string", "cv_fs_load_namespace", "cv_fs_load_namespace_string", "cv_fs_close", "cv_fs_wait_registered", "cv_fs_preregister", "cv_fs_arena_stats", "cv_synth_delete_file", "cv_worker_arena_stats", "cv_gpu_numa_node", "cv_gds_info", "cv_fs_metrics", "cv_fs_pool_stats",
            "cv_open", "cv_read", "cv_read_buf", "cv_read_full", "cv_fuse_read", "cv_seek", "cv_pos", "cv_len",
-           "cv_chunk_size", "cv_close_reader", "cv_read_device", "cv_read_device_sharded", "cv_read_many_device", "cv_shard_plan", "cv_readv_device", "cv_readv_plan", "cv_readv_strided_device", "cv_readv_strided_plan", "cv_readv_cast_device", "cv_readv_cast_plan", "cv_fuse_read_device", "cv_fuse_read_file_device",
+           "cv_chunk_size", "cv_close_reader", "cv_read_device", "cv_read_device_sharded", "cv_read_many_device", "cv_shard_plan", "cv_readv_device", "cv_readv_plan", "cv_readv_strided_device", "cv_readv_strided_plan", "cv_readv_cast_device", "cv_readv_cast_plan", "cv_readv_scaled_device", "cv_fuse_read_device", "cv_fuse_read_file_device",
            "cv_verify", "cv_device_stats", "cv_writer_open", "cv_write", "cv_write_device", "cv_writer_close", "cv_worker_start", "cv_worker_stop", "cv_worker_hbm_load", "cv_worker_hbm_drain", "cv_worker_hbm_stats", "cv_worker_hbm_tier", "cv_worker_metrics",
            "cv_synth_create_file", "cv_synth_set_shard_world", "cv_synth_block", "cv_host_crc",
            "cvh_pinned_alloc", "cvh_pinned_free", "cvh_host_register", "cvh_host_unregister", "cvh_device_alloc", "cvh_device_free", "cvh_h2d_async", "cvh_d2h_async", "cvh_stream_create", "cvh_stream_destroy",

@@ -362,6 +362,17 @@ static std::vector<ReadvRange> cast_ranges(const CvCastRange* ranges, int32_t n)
     return out;
 }
 
+static std::vector<ReadvRange> scaled_ranges(const CvScaledRange* ranges, int32_t n) {
+    std::vector<ReadvRange> out;
+    for (int32_t i = 0; ranges && i < n; i++) {
+        const CvScaledRange& s = ranges[i];
+        const CvCastRange& c = s.cast;
+        out.push_back(ReadvRange{c.file_off, c.row_len, static_cast<uint8_t*>(c.d_dst), c.rows, c.file_pitch, c.dst_pitch, c.src_dtype, c.dst_dtype,
+                                 ReadvScale{s.d_scale, s.scale_dtype, s.scale_rows, s.scale_cols, s.block_rows, s.block_cols, s.cols, s.first_elem}});
+    }
+    return out;
+}
+
 static int64_t readv_device_common(cv_reader* r, const std::vector<ReadvRange>& rs, int32_t n, cv_stream_t stream, int64_t* nbytes) {
     API_TRY(ensure_dev(r));
     int64_t got = 0;
@@ -440,6 +451,15 @@ int64_t cv_readv_cast_device(cv_reader* r, const CvCastRange* ranges, int32_t n,
     API_NEED(nbytes);
     if (n > 0) API_NEED(ranges);
     return readv_device_common(r, cast_ranges(ranges, n), n, stream, nbytes);
+    API_GUARD_END
+}
+
+int64_t cv_readv_scaled_device(cv_reader* r, const CvScaledRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes) {
+    API_GUARD_BEGIN
+    API_NEED(r);
+    API_NEED(nbytes);
+    if (n > 0) API_NEED(ranges);
+    return readv_device_common(r, scaled_ranges(ranges, n), n, stream, nbytes);
     API_GUARD_END
 }
 
@@ -933,6 +953,11 @@ __attribute__((weak)) int cvk_gather_strided(const uint8_t*, const CvStridedSeg*
 
 // The same for the cast gather of cast reads (cv_readv_cast_device).
 __attribute__((weak)) int cvk_gather_cast(const uint8_t*, const CvCastSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) {
+    return n ? int(cudaErrorNotSupported) : 0;
+}
+
+// And for K5's scaled instance (FP8 sources and scales of cv_readv_scaled_device / cv_readv_cast_device).
+__attribute__((weak)) int cvk_gather_cast_scaled(const uint8_t*, const CvCastSeg*, const CvScaleSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) {
     return n ? int(cudaErrorNotSupported) : 0;
 }
 

@@ -351,15 +351,49 @@ Err GpuFsReader::read_device_sharded(int rank, int world, void* d_dst, int64_t c
     return Err::ok();
 }
 
-static int64_t dtype_size(int32_t dt) { return dt == CV_DTYPE_F32 ? 4 : dt == CV_DTYPE_NONE ? 1 : 2; }
+static bool is_f8(int32_t dt) { return dt == CV_DTYPE_F8_E4M3 || dt == CV_DTYPE_F8_E5M2; }
+static int64_t dtype_size(int32_t dt) { return dt == CV_DTYPE_F32 ? 4 : dt == CV_DTYPE_NONE || is_f8(dt) ? 1 : 2; }
 
 // A range's destination row in bytes: row_len converted to the destination element size.
 static int64_t dst_row_len(const ReadvRange& r) { return r.cast() ? r.row_len / dtype_size(r.src_dtype) * dtype_size(r.dst_dtype) : r.row_len; }
 
+// The rules only a scaled range has (check_cast, after its element alignment was checked): the scale geometry covers every element
+// the range touches, without an int64 overflow anywhere.
+static Err check_scale(const ReadvRange& r, int32_t i) {
+    const ReadvScale& s = r.scale;
+    if (s.dtype != CV_DTYPE_F32 && s.dtype != CV_DTYPE_F16 && s.dtype != CV_DTYPE_BF16)
+        return Err::common(str_printf("readv: range %d has an unknown scale dtype code %d", i, s.dtype));
+    if (s.block_rows < 1 || s.block_cols < 1 || s.view_cols < 1 || s.rows < 1 || s.cols < 1)
+        return Err::common(str_printf("readv: range %d: block_rows, block_cols, cols, scale_rows and scale_cols must be at least 1", i));
+    if (s.first_elem < 0) return Err::common(str_printf("readv: range %d has a negative first_elem (%lld)", i, (long long)s.first_elem));
+    const int64_t need = s.view_cols / s.block_cols + (s.view_cols % s.block_cols != 0);
+    if (s.cols < need)
+        return Err::common(str_printf("readv: range %d: scale_cols %lld < ceil(cols / block_cols) = %lld", i, (long long)s.cols, (long long)need));
+    int64_t bytes;
+    if (__builtin_mul_overflow(s.rows, s.cols, &bytes) || __builtin_mul_overflow(bytes, dtype_size(s.dtype), &bytes))
+        return Err::common(str_printf("readv: range %d: scale_rows * scale_cols * scale size overflows", i));
+    if (r.rows == 0 || r.row_len == 0) return Err::ok();
+    // the last view element the range touches: first_elem + (rows - 1) * file_pitch / src size + row_len / src size - 1
+    const int64_t ss = dtype_size(r.src_dtype);
+    int64_t last;
+    if (__builtin_mul_overflow(r.rows - 1, r.rows > 1 ? r.file_pitch / ss : 0, &last) || __builtin_add_overflow(last, r.row_len / ss - 1, &last) ||
+        __builtin_add_overflow(last, s.first_elem, &last))
+        return Err::common(str_printf("readv: range %d: its last view element overflows int64", i));
+    const int64_t srow = last / s.view_cols / s.block_rows;
+    if (srow >= s.rows)
+        return Err::common(str_printf("readv: range %d: view element %lld maps to scale row %lld, but the scale has %lld rows", i, (long long)last,
+                                      (long long)srow, (long long)s.rows));
+    return Err::ok();
+}
+
 // The rules only a converting range has (plan_readv)
 static Err check_cast(const FileBlocks& fb, const ReadvRange& r, int32_t i) {
     for (int32_t dt : {r.src_dtype, r.dst_dtype})
-        if (dt < CV_DTYPE_NONE || dt > CV_DTYPE_BF16) return Err::common(str_printf("readv: range %d has an unknown dtype code %d", i, dt));
+        if (dt < CV_DTYPE_NONE || dt > CV_DTYPE_F8_E5M2) return Err::common(str_printf("readv: range %d has an unknown dtype code %d", i, dt));
+    if (r.scaled() && !is_f8(r.src_dtype))
+        return Err::common(str_printf("readv: range %d is scaled but its source dtype %d is not F8_E4M3 or F8_E5M2", i, r.src_dtype));
+    if (is_f8(r.dst_dtype) && (r.cast() || r.scaled()))
+        return Err::common(str_printf("readv: range %d converts to F8 dtype %d: F8 is a source type only", i, r.dst_dtype));
     if (!r.cast()) return Err::ok();
     if (r.src_dtype == CV_DTYPE_NONE || r.dst_dtype == CV_DTYPE_NONE)
         return Err::common(str_printf("readv: range %d converts dtype %d to %d: conversions are between F32, F16 and BF16 only", i, r.src_dtype, r.dst_dtype));
@@ -371,7 +405,7 @@ static Err check_cast(const FileBlocks& fb, const ReadvRange& r, int32_t i) {
     if (fb.status.block_size % ss)
         return Err::common(str_printf("readv: range %d: the file's block size %lld is not a multiple of the source element size (%lld)", i,
                                       (long long)fb.status.block_size, (long long)ss));
-    return Err::ok();
+    return r.scaled() ? check_scale(r, i) : Err::ok();
 }
 
 Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::vector<ReadvBlock>* blocks, std::vector<ReadvSpan>* spans) {
@@ -625,17 +659,19 @@ enum JobMode : uint8_t { kPlain = 0, kFramed = 1, kHole = 3 };
 
 // Layout of the per-call device tables (shared by all readers of the context) and of their pinned host image:
 //   off[J] len[J] expect[J] skip[J] | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F] | segs[n_segs] | strided[n_strided] | casts[n_casts]
+//   | scales[n_scales]
 // off .. skip are uploaded before the fetch starts; crc .. ferr are the results copied back.
 struct TableLayout {
-    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, o_segs = 0, o_strided = 0, o_casts = 0, bytes = 0;
+    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, o_segs = 0, o_strided = 0, o_casts = 0, o_scales = 0, bytes = 0;
     TableLayout() = default;
-    TableLayout(size_t j, size_t f, size_t n_segs, size_t n_strided, size_t n_casts) : J(j), F(f) {
+    TableLayout(size_t j, size_t f, size_t n_segs, size_t n_strided, size_t n_casts, size_t n_scales) : J(j), F(f) {
         auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
         o_len = up(8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_crc = up(o_skip + J);
         o_streams = up(o_crc + 4 * res_words()), o_fdesc = up(o_streams + sizeof(CvStreamDesc) * J);
         o_segs = up(o_fdesc + sizeof(CvFrameDesc) * F), o_strided = up(o_segs + sizeof(CvSeg) * n_segs);
         o_casts = up(o_strided + sizeof(CvStridedSeg) * n_strided);
-        bytes = up(o_casts + sizeof(CvCastSeg) * n_casts);
+        o_scales = up(o_casts + sizeof(CvCastSeg) * n_casts);
+        bytes = up(o_scales + sizeof(CvScaleSeg) * n_scales);
     }
     size_t res_words() const { return J + 4 + F; }
     uint64_t* off(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t); }
@@ -649,6 +685,7 @@ struct TableLayout {
     CvSeg* segs(uint8_t* t) const { return reinterpret_cast<CvSeg*>(t + o_segs); }
     CvStridedSeg* strided(uint8_t* t) const { return reinterpret_cast<CvStridedSeg*>(t + o_strided); }
     CvCastSeg* casts(uint8_t* t) const { return reinterpret_cast<CvCastSeg*>(t + o_casts); }
+    CvScaleSeg* scales(uint8_t* t) const { return reinterpret_cast<CvScaleSeg*>(t + o_scales); }
 };
 
 // What one run_jobs call does, decided before any CUDA call.
@@ -668,7 +705,7 @@ struct GpuFsReader::CallPlan {
     TableLayout tl;
 };
 
-Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, size_t n_casts, CallPlan* out) const {
+Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, size_t n_casts, size_t n_scales, CallPlan* out) const {
     CallPlan& P = *out;
     const B200Conf& bc = ctx_->conf.b200;
     const size_t J = jobs.size();
@@ -714,7 +751,7 @@ Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n
     P.group_verbatim.assign(P.NG, 0);
     for (size_t j = 0; j < J; j++) P.group_verbatim[j / P.k] |= P.mode[j] == kFramed;
     P.T_threads = static_cast<int>(std::min<size_t>(static_cast<size_t>(std::max(1, bc.fetch_threads)), P.NG));
-    P.tl = TableLayout(J, P.F, n_segs, n_strided, n_casts);
+    P.tl = TableLayout(J, P.F, n_segs, n_strided, n_casts, n_scales);
     return Err::ok();
 }
 
@@ -1067,9 +1104,10 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     const B200Conf& bc = ctx_->conf.b200;
     const int poly = bc.verify_poly ? 1 : 0;
     const size_t n_segs = pages ? pages->segs.size() : 0, n_strided = pages ? pages->strided.size() : 0, n_casts = pages ? pages->casts.size() : 0;
+    const size_t n_scales = pages ? pages->scales.size() : 0;
 
     CallPlan P;
-    CV_RETURN_IF_ERR(plan_call(jobs, n_segs, n_strided, n_casts, &P));
+    CV_RETURN_IF_ERR(plan_call(jobs, n_segs, n_strided, n_casts, n_scales, &P));
     Call c(*this, jobs, P, d_dst);
     if (!(bc.zero_copy && !P.call_framed)) CV_RETURN_IF_ERR(c.ensure_ring());
 
@@ -1108,6 +1146,10 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     if (n_casts) {  // and its table of cast segments
         memcpy(tl.casts(h), pages->casts.data(), sizeof(CvCastSeg) * n_casts);
         CU_TRY(cudaMemcpyAsync(tl.casts(T), tl.casts(h), sizeof(CvCastSeg) * n_casts, cudaMemcpyHostToDevice, G.vstream));
+    }
+    if (n_scales) {  // and the cast segments' scales, when K5's scaled instance runs
+        memcpy(tl.scales(h), pages->scales.data(), sizeof(CvScaleSeg) * n_scales);
+        CU_TRY(cudaMemcpyAsync(tl.scales(T), tl.scales(h), sizeof(CvScaleSeg) * n_scales, cudaMemcpyHostToDevice, G.vstream));
     }
     CU_TRY(cudaMemsetAsync(tl.crc(T), 0, 4 * tl.res_words(), G.vstream));
     CvStreamDesc* sd = tl.streams(h);
@@ -1186,7 +1228,9 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
         CVK_TRY(cvk_gather_pages(d_dst, tl.segs(T), static_cast<uint32_t>(n_segs), pages->total, pages->d_out, G.vstream));
     if (n_strided)  // spans of several rows each
         CVK_TRY(cvk_gather_strided(d_dst, tl.strided(T), static_cast<uint32_t>(n_strided), pages->strided_total, pages->d_out, G.vstream));
-    if (n_casts)  // spans of converting ranges: K5 out of the verified staging
+    if (n_casts && n_scales)  // spans of converting ranges, FP8 or scaled among them: K5's scaled instance out of the verified staging
+        CVK_TRY(cvk_gather_cast_scaled(d_dst, tl.casts(T), tl.scales(T), static_cast<uint32_t>(n_casts), pages->cast_elems, pages->d_out, G.vstream));
+    else if (n_casts)  // spans of converting ranges: K5 out of the verified staging
         CVK_TRY(cvk_gather_cast(d_dst, tl.casts(T), static_cast<uint32_t>(n_casts), pages->cast_elems, pages->d_out, G.vstream));
     CU_TRY(cudaMemcpyAsync(G.h_result, d_crc, 4 * tl.res_words(), cudaMemcpyDeviceToHost, G.vstream));
     CU_TRY(cudaEventRecord(G.done_ev, G.vstream));
@@ -1251,6 +1295,12 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
         CV_RETURN_IF_ERR(check_device_dst(r.dst, G.device).ctx(str_printf("range %d", i)));
         const int64_t dst_row = dst_row_len(r);
         CV_RETURN_IF_ERR(check_device_dst(r.dst + (r.rows - 1) * r.dst_pitch + dst_row - 1, G.device).ctx(str_printf("range %d (last byte)", i)));
+        if (r.scaled()) {  // the scale buffer too: its first and last byte (check_scale bounded its size)
+            const uint8_t* sp = static_cast<const uint8_t*>(r.scale.ptr);
+            CV_RETURN_IF_ERR(check_device_dst(sp, G.device).ctx(str_printf("range %d scale", i)));
+            CV_RETURN_IF_ERR(check_device_dst(sp + r.scale.rows * r.scale.cols * dtype_size(r.scale.dtype) - 1, G.device)
+                                 .ctx(str_printf("range %d scale (last byte)", i)));
+        }
         lo = std::min(lo, reinterpret_cast<uintptr_t>(r.dst));
         total += r.rows * dst_row;
     }
@@ -1281,6 +1331,7 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
     do {
         Scatter sc;
         sc.d_out = base;
+        bool any_scaled = false;  // a cast span of this round has an FP8 source or a scale
         for (size_t slot = 0; slot < per_round && next < boundary.size(); slot++, next++) {
             const ReadvBlock& b = blocks[boundary[next]];
             const int64_t at = rel(stage + slot * static_cast<size_t>(stage_block));
@@ -1295,6 +1346,14 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
                                                  sc.cast_chunks, r.src_dtype, r.dst_dtype});
                     sc.cast_elems += elems * rows;
                     sc.cast_chunks += rows * CV_CAST_ROW_CHUNKS(elems);
+                    // the view position of the span's first element: first_elem + (its file offset - file_off) / src size
+                    const ReadvScale& g = r.scale;
+                    const int64_t ss = dtype_size(r.src_dtype), at_file = fb.starts[b.block] + s.block_off;
+                    sc.scales.push_back(r.scaled() ? CvScaleSeg{g.ptr, uint64_t(g.block_rows), uint64_t(g.block_cols), uint64_t(g.cols),
+                                                                uint64_t(g.view_cols), uint64_t(g.first_elem + (at_file - r.file_off) / ss),
+                                                                uint64_t(r.file_pitch / ss), g.dtype, 0}
+                                                   : CvScaleSeg{});
+                    any_scaled |= r.scaled() || is_f8(r.src_dtype);
                 } else if (s.rows == 1) {
                     sc.segs.push_back(CvSeg{src, dst, len});
                     sc.total += len;
@@ -1304,6 +1363,7 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
                 }
             }
         }
+        if (!any_scaled) sc.scales.clear();  // plain K5, exactly as without scales
         CV_RETURN_IF_ERR(run_jobs(jobs, base, stream, sc.segs.empty() && sc.strided.empty() && sc.casts.empty() ? nullptr : &sc));
         jobs.clear();
     } while (next < boundary.size());

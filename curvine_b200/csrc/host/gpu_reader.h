@@ -53,12 +53,20 @@ Err plan_shard(const FileBlocks& fb, int rank, int world, int64_t cap, std::vect
 // verified there like any whole block, and its spans are delivered from the staging by K3.  A range whose src_dtype differs from its
 // dst_dtype converts its elements (CV_DTYPE_*): its file side is in source bytes, its destination side (dst, dst_pitch, a span's dst_off)
 // in destination bytes, and none of the blocks it touches is direct, so each is verified before K5 converts it out of the staging.
+// A scaled range (scale.ptr != nullptr, FP8 sources only) also multiplies every element by its scale (CvScaledRange).
+struct ReadvScale {
+    const void* ptr = nullptr;
+    int32_t dtype = CV_DTYPE_NONE;
+    int64_t rows = 0, cols = 0, block_rows = 0, block_cols = 0, view_cols = 0, first_elem = 0;
+};
 struct ReadvRange {
     int64_t file_off, row_len;
     uint8_t* dst;
     int64_t rows = 1, file_pitch = 0, dst_pitch = 0;  // the pitches only matter when rows > 1
     int32_t src_dtype = CV_DTYPE_NONE, dst_dtype = CV_DTYPE_NONE;
+    ReadvScale scale;
     bool cast() const { return src_dtype != dst_dtype; }
+    bool scaled() const { return scale.ptr != nullptr; }
 };
 struct ReadvSpan {
     int64_t block_off, len;  // row k < rows of the span: bytes [block_off + k*file_pitch, +len) of the block
@@ -77,7 +85,7 @@ struct ReadvBlock {
 // clipped first row, the whole rows, a clipped last row), computed without visiting the rows: O(ranges + touched blocks).  A converting
 // range is an error besides when a dtype code is unknown, when it converts to or from CV_DTYPE_NONE, when an element could straddle two
 // blocks or a source or destination element is misaligned (see cv_readv_cast_device), or when its dst_pitch is shorter than its
-// destination row.
+// destination row.  A scaled range is an error besides for the rules of cv_readv_scaled_device (all but the device-memory check).
 Err plan_readv(const FileBlocks& fb, const ReadvRange* ranges, int32_t n, std::vector<ReadvBlock>* blocks, std::vector<ReadvSpan>* spans);
 
 class GpuIngest;  // per-FsContext pinned ring + streams
@@ -125,7 +133,8 @@ class GpuFsReader {
     // scatter riding on a read: after the bytes landed in d_dst and were CRC'd, segs[i] copies d_dst + src_off to d_out + dst_off
     // (K3), in the same launch train, no extra sync.  Page buffers of a FUSE reply (Reader::fuse_read + ResponseData::as_iovec on the
     // device), or the spans of the boundary blocks of a vectored read: one-row spans as segs (K3), spans of several rows as strided
-    // (K3 over 2D descriptors), spans of converting ranges as casts (K5).
+    // (K3 over 2D descriptors), spans of converting ranges as casts (K5).  When a cast span has an FP8 source or a scale, `scales`
+    // holds one CvScaleSeg per cast (null scale for the others) and K5's scaled instance runs instead; otherwise `scales` is empty.
     struct Scatter {
         uint8_t* d_out = nullptr;
         std::vector<CvSeg> segs;
@@ -134,10 +143,11 @@ class GpuFsReader {
         uint64_t strided_total = 0;  // sum of strided[i].len * strided[i].rows
         std::vector<CvCastSeg> casts;
         uint64_t cast_elems = 0, cast_chunks = 0;  // sum of casts[i].elems * rows, and the next segment's `first`
+        std::vector<CvScaleSeg> scales;
     };
     struct CallPlan;  // what one run_jobs call does, decided up front (plan_call)
     struct Call;      // one run_jobs call in flight: fetch workers and the ingest paths of a copy group
-    Err plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, size_t n_casts, CallPlan* out) const;
+    Err plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, size_t n_casts, size_t n_scales, CallPlan* out) const;
     Err run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* stream, const Scatter* scatter = nullptr);
     Err read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const Scatter* scatter);
     FsContext* ctx_ = nullptr;

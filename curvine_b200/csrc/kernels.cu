@@ -19,6 +19,7 @@
 
 #include <atomic>
 #include <cstdlib>
+#include <cstring>
 #include <mutex>
 #include <vector>
 
@@ -934,12 +935,147 @@ __device__ __forceinline__ void ld_chunk(const uint8_t* p, uint32_t size, uint32
     }
 }
 
+// ---- the scaled instance's additions: FP8 sources and a scale per element
+// The FP8 decoders are branch-free (selects, no normalisation loop): a warp's 8 x 32 elements mix subnormals with normals.
+
+__device__ __forceinline__ uint32_t small_to_f32(uint32_t m) {  // F32 bits of the integer m < 2^24: exact
+#if defined(__CUDA_ARCH__)
+    return __float_as_uint(__uint2float_rn(m));
+#else
+    const float x = static_cast<float>(m);
+    memcpy(&m, &x, 4);
+    return m;
+#endif
+}
+
+__device__ __forceinline__ uint32_t e4m3_to_f32(uint32_t b) {  // exact; no infinities, 0x7f / 0xff are NaN
+    const uint32_t sign = (b & 0x80u) << 24, a = b & 0x7fu;
+    if (a == 0x7fu) return sign | 0x7fc00000u;
+    // normal: exponent e + 120, mantissa m, i.e. (a + (120 << 3)) << 20; subnormal m * 2^-9: the float m with 9 off its exponent
+    return sign | (a >= 8u ? (a + 0x3c0u) << 20 : a ? small_to_f32(a) - (9u << 23) : 0u);
+}
+
+__device__ __forceinline__ uint32_t e5m2_to_f32(uint32_t b) {  // exact; the top byte of an F16
+    const uint32_t sign = (b & 0x80u) << 24, a = b & 0x7fu;
+    if (a >= 0x7cu) return sign | 0x7f800000u | ((a & 3u) << 21);  // inf, NaN (payload kept)
+    // normal: exponent e + 112, i.e. (a + (112 << 2)) << 21; subnormal m * 2^-16
+    return sign | (a >= 4u ? (a + 0x1c0u) << 21 : a ? small_to_f32(a) - (16u << 23) : 0u);
+}
+
+__device__ __forceinline__ bool is_f8(int32_t dt) { return dt == CV_DTYPE_F8_E4M3 || dt == CV_DTYPE_F8_E5M2; }
+
+// any source element -> F32 bits, exact
+__device__ __forceinline__ uint32_t to_f32(uint32_t v, int32_t sdt) {
+    return sdt == CV_DTYPE_F8_E4M3 ? e4m3_to_f32(v) : sdt == CV_DTYPE_F8_E5M2 ? e5m2_to_f32(v) : sdt == CV_DTYPE_F16 ? f16_to_f32(v)
+         : sdt == CV_DTYPE_BF16 ? v << 16 : v;
+}
+
+__device__ __forceinline__ uint32_t from_f32(uint32_t f, int32_t ddt) {
+    return ddt == CV_DTYPE_F16 ? f32_to_f16(f) : ddt == CV_DTYPE_BF16 ? f32_to_bf16(f) : f;
+}
+
+// one IEEE F32 multiply, round-to-nearest-even, never contracted into an FMA
+__device__ __forceinline__ uint32_t f32_mul(uint32_t a, uint32_t b) {
+#if defined(__CUDA_ARCH__)
+    return __float_as_uint(__fmul_rn(__uint_as_float(a), __uint_as_float(b)));
+#else
+    float x, y;
+    memcpy(&x, &a, 4), memcpy(&y, &b, 4);
+    x *= y;
+    memcpy(&a, &x, 4);
+    return a;
+#endif
+}
+
+// 8 FP8 elements from p: one 8-byte load when p is 8-byte aligned, bytes otherwise
+__device__ __forceinline__ void ld_chunk8(const uint8_t* p, uint32_t v[8]) {
+    if ((reinterpret_cast<uintptr_t>(p) & 7u) == 0) {
+        const uint64_t w = *reinterpret_cast<const uint64_t*>(p);
+#pragma unroll
+        for (int k = 0; k < 8; k++) v[k] = static_cast<uint32_t>(w >> (8 * k)) & 0xffu;
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; k++) v[k] = p[k];
+    }
+}
+
+// a / b, in 32 bits when both fit (every tensor below 2^32 elements): the 64-bit division is a long software sequence
+__device__ __forceinline__ uint64_t udiv(uint64_t a, uint64_t b) { return (a | b) >> 32 ? a / b : uint64_t(uint32_t(a) / uint32_t(b)); }
+
+// The scale of the element in hand, kept in a register and stepped element by element: (i, j) is the element's view position, as
+// (ib, ir) = divmod(i, block_rows) and (jb, jr) = divmod(j, block_cols).  Found by division once per chunk (start), then only
+// compared and incremented; the scale is reloaded when the element enters another tile.  No scale table entry: s = 1.0 (exact).
+// step() moves to the NEXT element and loads its scale, so it is called only when that element exists (before every element but the
+// first): stepping past the range's last element could address a scale beyond the caller's buffer (the last view row of a per-tensor,
+// per-row or whole-tile grid wraps into scale row scale_rows).
+struct ScaleWalk {
+    const uint8_t* p;
+    int32_t dt;
+    uint64_t cols, br, bc, scols, j, jr, jb, ir, ib;
+    uint32_t s;
+    __device__ __forceinline__ void load() {
+        const uint64_t q = ib * scols + jb;
+        s = dt == CV_DTYPE_F32 ? __ldg(reinterpret_cast<const uint32_t*>(p) + q)
+          : dt == CV_DTYPE_F16 ? f16_to_f32(__ldg(reinterpret_cast<const uint16_t*>(p) + q))
+                               : uint32_t(__ldg(reinterpret_cast<const uint16_t*>(p) + q)) << 16;
+    }
+    __device__ __forceinline__ void start(const CvScaleSeg& g, uint64_t row, uint64_t e) {
+        p = static_cast<const uint8_t*>(g.scale);
+        s = 0x3f800000u;
+        if (!p) return;
+        dt = g.scale_dtype, cols = g.cols, br = g.block_rows, bc = g.block_cols, scols = g.scale_cols;
+        const uint64_t v = g.view0 + row * g.view_step + e, i = udiv(v, cols);
+        j = v - i * cols, ib = udiv(i, br), ir = i - ib * br, jb = udiv(j, bc), jr = j - jb * bc;
+        load();
+    }
+    __device__ __forceinline__ bool flat(uint32_t m) const { return !p || (jr + m <= bc && j + m <= cols); }  // the next m share s
+    __device__ __forceinline__ void step() {
+        if (!p) return;
+        if (++j == cols) {
+            j = jr = jb = 0;
+            if (++ir == br) ir = 0, ib++;
+            load();
+        } else if (++jr == bc) {
+            jr = 0, jb++;
+            load();
+        }
+    }
+};
+
+// A whole chunk through F32 with its scales.  Called with constant dtypes for the FP8 pairs (scale_chunk), so each pair inlines to
+// straight-line code with no per-element dtype selects.
+__device__ __forceinline__ void scale8(uint32_t v[8], int32_t sdt, int32_t ddt, ScaleWalk& w) {
+    if (w.flat(8)) {  // one scale for the chunk
+#pragma unroll
+        for (int j = 0; j < 8; j++) v[j] = from_f32(f32_mul(to_f32(v[j], sdt), w.s), ddt);
+    } else {  // the chunk crosses a tile edge or a view row
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            if (j) w.step();
+            v[j] = from_f32(f32_mul(to_f32(v[j], sdt), w.s), ddt);
+        }
+    }
+}
+
+__device__ __forceinline__ void scale_chunk(uint32_t v[8], int32_t sdt, int32_t ddt, ScaleWalk& w) {
+    if (sdt == CV_DTYPE_F8_E4M3 && ddt == CV_DTYPE_BF16) scale8(v, CV_DTYPE_F8_E4M3, CV_DTYPE_BF16, w);
+    else if (sdt == CV_DTYPE_F8_E4M3 && ddt == CV_DTYPE_F16) scale8(v, CV_DTYPE_F8_E4M3, CV_DTYPE_F16, w);
+    else if (sdt == CV_DTYPE_F8_E4M3) scale8(v, CV_DTYPE_F8_E4M3, CV_DTYPE_F32, w);
+    else if (sdt == CV_DTYPE_F8_E5M2 && ddt == CV_DTYPE_BF16) scale8(v, CV_DTYPE_F8_E5M2, CV_DTYPE_BF16, w);
+    else if (sdt == CV_DTYPE_F8_E5M2 && ddt == CV_DTYPE_F16) scale8(v, CV_DTYPE_F8_E5M2, CV_DTYPE_F16, w);
+    else if (sdt == CV_DTYPE_F8_E5M2) scale8(v, CV_DTYPE_F8_E5M2, CV_DTYPE_F32, w);
+    else scale8(v, sdt, ddt, w);  // a scaled F32 / F16 / BF16 segment
+}
+
 // Grid-stride over the work chunks of all segments (CvCastSeg::first numbers them): neighbouring threads take neighbouring chunks, so
 // every load and store of a warp is coalesced whatever the shape.  In a row whose destination is `head` elements short of a 16-byte
 // boundary, chunk 0 holds those head elements and chunk k >= 1 the 8 elements from head + 8(k-1) on (with head = 0, chunk k holds 8k..):
 // every whole chunk stores one (2-byte destination) or two (4-byte destination) aligned 16-byte vectors.
+// SCALED (cvk_gather_cast_scaled) adds FP8 sources and scales[]; the plain instance never reads `scales` and compiles to the code it
+// compiled to before the scaled one existed.
+template <bool SCALED>
 __global__ void __launch_bounds__(256) gather_cast_kernel(const uint8_t* __restrict__ src, const CvCastSeg* __restrict__ segs, uint32_t n,
-                                                          uint8_t* __restrict__ dst) {
+                                                          uint8_t* __restrict__ dst, const CvScaleSeg* __restrict__ scales) {
     const uint64_t total = segs[n - 1].first + segs[n - 1].rows * CV_CAST_ROW_CHUNKS(segs[n - 1].elems);
     uint32_t d = 0;  // the segment of the previous chunk: chunks only grow, so the search starts there
     for (uint64_t c = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; c < total; c += uint64_t(gridDim.x) * blockDim.x) {
@@ -956,9 +1092,13 @@ __global__ void __launch_bounds__(256) gather_cast_kernel(const uint8_t* __restr
         const uint64_t cpr = CV_CAST_ROW_CHUNKS(s.elems), rel = c - s.first;
         if (c < s.first || rel >= s.rows * cpr) continue;  // a table whose `first` leaves gaps: nothing is written outside a row
         const int32_t sdt = s.src_dtype, ddt = s.dst_dtype;
-        if ((sdt != CV_DTYPE_F32 && sdt != CV_DTYPE_F16 && sdt != CV_DTYPE_BF16) || (ddt != CV_DTYPE_F32 && ddt != CV_DTYPE_F16 && ddt != CV_DTYPE_BF16))
+        const bool f8 = SCALED && is_f8(sdt);
+        if ((!f8 && sdt != CV_DTYPE_F32 && sdt != CV_DTYPE_F16 && sdt != CV_DTYPE_BF16) ||
+            (ddt != CV_DTYPE_F32 && ddt != CV_DTYPE_F16 && ddt != CV_DTYPE_BF16))
             continue;
-        const uint32_t ss = cast_size(sdt), ds = cast_size(ddt);
+        // through F32 with a multiply: FP8 sources and scaled segments (the scale is 1.0 for an unscaled FP8 one)
+        const bool mul = SCALED && (f8 || scales[d].scale);
+        const uint32_t ss = f8 ? 1u : cast_size(sdt), ds = cast_size(ddt);
         const uint64_t row = rel < cpr ? 0 : rel / cpr, k = rel - row * cpr;
         const uint8_t* sp = src + s.src_off + row * s.src_pitch;
         uint8_t* dp = dst + s.dst_off + row * s.dst_pitch;
@@ -966,11 +1106,18 @@ __global__ void __launch_bounds__(256) gather_cast_kernel(const uint8_t* __restr
         const int64_t e0 = 8 * int64_t(k) - int64_t((8u - head) & 7u);  // chunk k: elements [e0, e0 + 8) of the row, clipped to it
         const int64_t lo = e0 > 0 ? e0 : 0, hi = e0 + 8 < int64_t(s.elems) ? e0 + 8 : int64_t(s.elems);
         if (lo >= hi) continue;
+        ScaleWalk w;
+        if (mul) w.start(scales[d], row, uint64_t(lo));
         if (hi - lo == 8) {  // a whole chunk: its destination is 16-byte aligned
             uint32_t v[8];
-            ld_chunk(sp + lo * ss, ss, v);
+            if (f8) ld_chunk8(sp + lo, v);
+            else ld_chunk(sp + lo * ss, ss, v);
+            if (!mul) {
 #pragma unroll
-            for (int j = 0; j < 8; j++) v[j] = cast_elem(v[j], sdt, ddt);
+                for (int j = 0; j < 8; j++) v[j] = cast_elem(v[j], sdt, ddt);
+            } else {
+                scale_chunk(v, sdt, ddt, w);
+            }
             uint4* o = reinterpret_cast<uint4*>(dp + lo * ds);
             if (ds == 2) {
                 st_vec(o, make_uint4(v[0] | v[1] << 16, v[2] | v[3] << 16, v[4] | v[5] << 16, v[6] | v[7] << 16));
@@ -978,8 +1125,14 @@ __global__ void __launch_bounds__(256) gather_cast_kernel(const uint8_t* __restr
                 st_vec(o, make_uint4(v[0], v[1], v[2], v[3]));
                 st_vec(o + 1, make_uint4(v[4], v[5], v[6], v[7]));
             }
-        } else {
+        } else if (!mul) {
             for (int64_t e = lo; e < hi; e++) st_elem(dp + e * ds, ds, cast_elem(ld_elem(sp + e * ss, ss), sdt, ddt));
+        } else {
+            for (int64_t e = lo; e < hi; e++) {
+                if (e > lo) w.step();
+                const uint32_t x = f8 ? uint32_t(sp[e]) : ld_elem(sp + e * ss, ss);
+                st_elem(dp + e * ds, ds, from_f32(f32_mul(to_f32(x, sdt), w.s), ddt));
+            }
         }
     }
 }
@@ -1390,7 +1543,9 @@ int cvk_gather_strided(const uint8_t* d_src, const CvStridedSeg* d_segs, uint32_
     return rc ? rc : int(freed);
 }
 
-int cvk_gather_cast(const uint8_t* d_src, const CvCastSeg* d_segs, uint32_t n, uint64_t total_elems, uint8_t* d_dst, cv_stream_t stream) {
+// K5, plain (d_scales == NULL) or scaled: one launch statement, the instance chosen through a function pointer
+static int launch_cast(const uint8_t* d_src, const CvCastSeg* d_segs, const CvScaleSeg* d_scales, uint32_t n, uint64_t total_elems, uint8_t* d_dst,
+                       cv_stream_t stream) {
     if (n == 0 || total_elems == 0) return 0;
     DeviceGuard guard(d_dst);
     int dev;
@@ -1398,9 +1553,20 @@ int cvk_gather_cast(const uint8_t* d_src, const CvCastSeg* d_segs, uint32_t n, u
     // the table stays on the device: the kernel takes the chunk count from its last entry.  One thread per 8 elements, at most 8
     // CTAs of 256 per SM; the grid-stride loop takes the rest (and the head chunks of many short rows).
     const uint64_t want = total_elems / (8 * 256) + 1, cap = uint64_t(g_sm_count[dev]) * 8;
-    gather_cast_kernel<<<uint32_t(want < cap ? want : cap), 256, 0, static_cast<cudaStream_t>(stream)>>>(d_src, d_segs, n, d_dst);
+    auto cast = d_scales ? gather_cast_kernel<true> : gather_cast_kernel<false>;
+    cast<<<uint32_t(want < cap ? want : cap), 256, 0, static_cast<cudaStream_t>(stream)>>>(d_src, d_segs, n, d_dst, d_scales);
     count_launch();
     return int(cudaGetLastError());
+}
+
+int cvk_gather_cast(const uint8_t* d_src, const CvCastSeg* d_segs, uint32_t n, uint64_t total_elems, uint8_t* d_dst, cv_stream_t stream) {
+    return launch_cast(d_src, d_segs, nullptr, n, total_elems, d_dst, stream);
+}
+
+int cvk_gather_cast_scaled(const uint8_t* d_src, const CvCastSeg* d_segs, const CvScaleSeg* d_scales, uint32_t n, uint64_t total_elems,
+                           uint8_t* d_dst, cv_stream_t stream) {
+    if (n && !d_scales) return int(cudaErrorInvalidValue);
+    return launch_cast(d_src, d_segs, d_scales, n, total_elems, d_dst, stream);
 }
 
 int cvk_deinterleave_blocks(const uint8_t* d_gathered, uint64_t shard_stride, uint32_t world, uint64_t block_size,

@@ -166,13 +166,15 @@ class CurvineClient:
         finally:
             reader.close()
 
-    def load_safetensors(self, path, device=None, names=None, slices=None, dtype=None):
+    def load_safetensors(self, path, device=None, names=None, slices=None, dtype=None, scales=None, scale_block=None):
         """Addition: a safetensors checkpoint as {name: CUDA tensor}, from one CRC-verified vectored read (curvine_b200.safetensors);
         slices = {name: (dim, start, stop)} loads only that part of a tensor (a tensor-parallel rank's shard); dtype converts the
-        float32, float16 and bfloat16 tensors to it on the GPU as they load."""
+        float32, float16 and bfloat16 tensors to it on the GPU as they load; scales = {float8 weight: its scale tensor} (and scale_block
+        for block scales) dequantizes those weights to dtype as they load."""
         from . import safetensors
         try:
-            return safetensors.load_file(self.file_system_ptr, path, device=device, names=names, slices=slices, dtype=dtype)
+            return safetensors.load_file(self.file_system_ptr, path, device=device, names=names, slices=slices, dtype=dtype, scales=scales,
+                                        scale_block=scale_block)
         except _fs.FsError as e:
             raise IOError("Native load safetensors failed: %s" % e)
 

@@ -237,29 +237,55 @@ class Reader:
         return spans, nb.value, fb.value
 
     @staticmethod
-    def _cast_ranges(ranges):
+    def _fill_cast(a, i, rng):
         import torch
-        codes = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.bfloat16: _lib.DTYPE_BF16}
+        off, row_len, rows, file_pitch, ptr, dst_pitch, src, dst = rng
+        floats = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.bfloat16: _lib.DTYPE_BF16}
+        f8 = {torch.float8_e4m3fn: _lib.DTYPE_F8_E4M3, torch.float8_e5m2: _lib.DTYPE_F8_E5M2}
+        if src == dst:
+            sc = dc = floats.get(src, f8.get(src, _lib.DTYPE_NONE))
+        elif (src in floats or src in f8) and dst in floats:
+            sc, dc = floats.get(src, f8.get(src)), floats[dst]
+        else:
+            raise ValueError("range %d: conversions are from float32, float16, bfloat16, float8_e4m3fn or float8_e5m2 to float32, float16 or "
+                             "bfloat16 only, not %s -> %s" % (i, src, dst))
+        a.file_off, a.row_len, a.rows, a.file_pitch, a.d_dst, a.dst_pitch = off, row_len, rows, file_pitch, ptr, dst_pitch
+        a.src_dtype, a.dst_dtype = sc, dc
+
+    @staticmethod
+    def _cast_ranges(ranges):
         arr = (_lib.CvCastRange * max(1, len(ranges)))()
-        for i, (off, row_len, rows, file_pitch, ptr, dst_pitch, src, dst) in enumerate(ranges):
-            if src == dst:
-                sc = dc = codes.get(src, _lib.DTYPE_NONE)
-            elif src in codes and dst in codes:
-                sc, dc = codes[src], codes[dst]
-            else:
-                raise ValueError("range %d: conversions are between float32, float16 and bfloat16 only, not %s -> %s" % (i, src, dst))
-            a = arr[i]
-            a.file_off, a.row_len, a.rows, a.file_pitch, a.d_dst, a.dst_pitch = off, row_len, rows, file_pitch, ptr, dst_pitch
-            a.src_dtype, a.dst_dtype = sc, dc
+        for i, rng in enumerate(ranges):
+            Reader._fill_cast(arr[i], i, rng)
         return arr
 
     def readv_cast_device(self, ranges, stream: int = 0) -> int:
         """Cast device read: `ranges` is a list of (file_off, row_len, rows, file_pitch, d_ptr, dst_pitch, src_dtype, dst_dtype) with torch
         dtypes.  A range with src_dtype == dst_dtype is a range of readv_strided_device; any other converts its elements on the GPU (float32,
-        float16 and bfloat16 into one another, round-to-nearest-even): its file side is in source bytes, d_ptr and dst_pitch in destination
+        float16 and bfloat16 into one another, round-to-nearest-even; float8_e4m3fn and float8_e5m2 into those three, exactly): its file side is in source bytes, d_ptr and dst_pitch in destination
         bytes.  Every block a converting range touches is verified before it is converted.  -> bytes delivered."""
         n = ctypes.c_int64()
         _check(_lib.lib().cv_readv_cast_device(self._h, self._cast_ranges(ranges), len(ranges), ctypes.c_void_p(stream), ctypes.byref(n)))
+        return n.value
+
+    def readv_scaled_device(self, ranges, stream: int = 0) -> int:
+        """Scaled device read (FP8 checkpoints): `ranges` is a list of readv_cast_device ranges with one more item, `scale`: None (the
+        range is a readv_cast_device range) or (d_ptr, dtype, scale_rows, scale_cols, block_rows, block_cols, cols, first_elem), the
+        scale_rows x scale_cols scales (torch dtype float32, float16 or bfloat16) of a float8_e4m3fn / float8_e5m2 weight seen as a
+        row-major view of `cols` columns.  View element (i, j) is multiplied by scale[i // block_rows, j // block_cols] in float32 and
+        rounded once to the range's result dtype; element e of range row k is view element first_elem + k * file_pitch + e.  -> bytes
+        delivered."""
+        import torch
+        scodes = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.bfloat16: _lib.DTYPE_BF16}
+        arr = (_lib.CvScaledRange * max(1, len(ranges)))()
+        for i, rng in enumerate(ranges):
+            a = arr[i]
+            self._fill_cast(a.cast, i, rng[:8])
+            if rng[8] is not None:
+                ptr, dt, a.scale_rows, a.scale_cols, a.block_rows, a.block_cols, a.cols, a.first_elem = rng[8]
+                a.d_scale, a.scale_dtype = ptr, scodes.get(dt, -1)
+        n = ctypes.c_int64()
+        _check(_lib.lib().cv_readv_scaled_device(self._h, arr, len(ranges), ctypes.c_void_p(stream), ctypes.byref(n)))
         return n.value
 
     def readv_cast_plan(self, ranges):

@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import CvCastSeg, CvFrameDesc, CvSeg, CvStreamDesc, CvStridedSeg, check
+from ._lib import CvCastSeg, CvFrameDesc, CvScaleSeg, CvSeg, CvStreamDesc, CvStridedSeg, check
 
 POLY_IEEE, POLY_CASTAGNOLI = 0, 1
 
@@ -123,6 +123,22 @@ def cast_segs_to_device(segs, device):
 
 def gather_cast(src, d_segs, n, total_elems, dst, stream=None):
     check(_lib.lib().cvk_gather_cast(_ptr(src), _ptr(d_segs), n, total_elems, _ptr(dst), _stream_ptr(stream)), "cvk_gather_cast")
+
+
+def scale_segs_to_device(scales, device):
+    """scales: one entry per cast segment, None (not scaled) or (scale_ptr, scale_dtype, block_rows, block_cols, scale_cols, cols, view0,
+    view_step) with a _lib.DTYPE_* scale dtype (see CvScaleSeg).  -> device table"""
+    arr = (CvScaleSeg * len(scales))()
+    for i, sc in enumerate(scales):
+        if sc is not None:
+            ptr, dt, br, bc, scols, cols, view0, step = sc
+            arr[i] = CvScaleSeg(ptr, br, bc, scols, cols, view0, step, dt, 0)
+    return _struct_array_to_device(arr, device)
+
+
+def gather_cast_scaled(src, d_segs, d_scales, n, total_elems, dst, stream=None):
+    check(_lib.lib().cvk_gather_cast_scaled(_ptr(src), _ptr(d_segs), _ptr(d_scales), n, total_elems, _ptr(dst), _stream_ptr(stream)),
+          "cvk_gather_cast_scaled")
 
 
 def deinterleave_blocks(gathered, shard_stride, world, block_size, n_blocks, file_len, dst, stream=None):

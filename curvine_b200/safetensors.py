@@ -113,10 +113,11 @@ def _is_integral(x) -> bool:
     return isinstance(x, numbers.Integral) and not isinstance(x, bool)
 
 
-def _cast_targets(data_start: int, entries: Dict[str, tuple], selected, dtype) -> Dict[str, object]:
+def _cast_targets(data_start: int, entries: Dict[str, tuple], selected, dtype, scaled=()) -> Dict[str, object]:
     """{name: dtype of the result} for load_file(dtype=...): the float32, float16 and bfloat16 tensors become `dtype`, the others stay as
     stored.  Raises ValueError for a target dtype other than those three, for a selected float tensor of another width (float64, float8:
-    not converted) and for a converting tensor whose data offset is not a multiple of its element size."""
+    not converted) and for a converting tensor whose data offset is not a multiple of its element size.  The float8 weights named in
+    `scaled` (load_file(scales=...)) become `dtype` too."""
     import torch
     floats = (torch.float32, torch.float16, torch.bfloat16)
     if dtype not in floats:
@@ -124,6 +125,9 @@ def _cast_targets(data_start: int, entries: Dict[str, tuple], selected, dtype) -
     out = {}
     for name in selected:
         stored, _, begin, end = entries[name]
+        if name in scaled:
+            out[name] = dtype
+            continue
         if stored.is_floating_point and stored not in floats:
             raise ValueError("%s: %s tensors are not converted on load (only float32, float16 and bfloat16 are)" % (name, stored))
         out[name] = dtype if stored in floats else stored
@@ -132,7 +136,57 @@ def _cast_targets(data_start: int, entries: Dict[str, tuple], selected, dtype) -
     return out
 
 
-def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=None, dtype=None) -> List[tuple]:
+def _scale_geometry(entries: Dict[str, tuple], selected, scales, scale_block, dtype) -> Dict[str, tuple]:
+    """{weight: (scale name, scale_rows, scale_cols, block_rows, block_cols, cols)} for the selected weights of load_file(scales=...).
+    The weight is seen as the row-major 2-D view [V_rows, cols = shape[-1]]; its scale is one element (per tensor, any shape), (V_rows, 1)
+    for a 2-D weight (per row), or, with scale_block = (br, bc), (ceil(R / br), ceil(C / bc)) for a 2-D weight (blocks).  Raises
+    ValueError, naming the weight and its scale, for anything else (see load_file)."""
+    import torch
+    if dtype is None:
+        raise ValueError("scales are given without dtype: dequantized weights need a result dtype")
+    if scale_block is not None and (not isinstance(scale_block, (tuple, list)) or len(scale_block) != 2
+                                    or not all(_is_integral(x) and x >= 1 for x in scale_block)):
+        raise ValueError("scale_block %r is not (block_rows, block_cols) of positive integers" % (scale_block,))
+    f8 = (torch.float8_e4m3fn, torch.float8_e5m2)
+    floats = (torch.float32, torch.float16, torch.bfloat16)
+    sel = set(selected)
+    out = {}
+    for w, sname in dict(scales).items():
+        if w not in entries:
+            raise ValueError("%s (scale %s): the file holds no such weight" % (w, sname))
+        if sname not in entries:
+            raise ValueError("%s: its scale %s is not in the file" % (w, sname))
+        if sname == w or sname in scales:
+            raise ValueError("%s: its scale %s is itself a weight named in scales" % (w, sname))
+        wdt, wshape, _, _ = entries[w]
+        sdt, sshape, _, _ = entries[sname]
+        if wdt not in f8:
+            raise ValueError("%s (scale %s): a scaled weight must be F8_E4M3 or F8_E5M2, not %s" % (w, sname, wdt))
+        if sdt not in floats:
+            raise ValueError("%s: its scale %s must be F32, F16 or BF16, not %s" % (w, sname, sdt))
+        if w not in sel:
+            continue
+        cols = wshape[-1] if wshape else 1
+        numel = 1
+        for x in wshape:
+            numel *= x
+        vrows = numel // cols if cols else 0
+        snumel = 1
+        for x in sshape:
+            snumel *= x
+        if snumel == 1:  # per tensor
+            out[w] = (sname, 1, 1, max(1, vrows), max(1, cols), max(1, cols))
+        elif len(wshape) == 2 and tuple(sshape) == (wshape[0], 1):  # per row
+            out[w] = (sname, wshape[0], 1, 1, max(1, cols), max(1, cols))
+        elif len(wshape) == 2 and scale_block is not None and tuple(sshape) == (-(-wshape[0] // scale_block[0]), -(-wshape[1] // scale_block[1])):
+            out[w] = (sname, sshape[0], sshape[1], int(scale_block[0]), int(scale_block[1]), max(1, cols))
+        else:
+            raise ValueError("%s %s: its scale %s has shape %s, which is neither one element, (rows, 1) of a 2-D weight nor the "
+                             "(ceil(R / br), ceil(C / bc)) blocks of scale_block=%s" % (w, tuple(wshape), sname, tuple(sshape), scale_block))
+    return out
+
+
+def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=None, dtype=None, scales=None, scale_block=None) -> List[tuple]:
     """The loader's ranges, without a GPU.  -> [(name, dtype, shape of the result, range)] for the selected names, in order, where range
     is (file_off, row_len, rows, file_pitch, dst_pitch) of Reader.readv_strided_device (d_ptr left out), or None when the tensor has no
     bytes to read.  An unsliced tensor is one row.  slices[name] = (dim, start, stop) keeps [start, stop) of dimension dim: the rows are
@@ -140,11 +194,18 @@ def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=Non
     apart (inner = prod(shape[dim+1:]) * itemsize), landing back to back.  With `dtype` (float32, float16 or bfloat16) the float32,
     float16 and bfloat16 tensors come back in `dtype`, the others as stored: dtype is the result's and range is (file_off, row_len, rows,
     file_pitch, dst_pitch, stored dtype, result dtype) of Reader.readv_cast_device, its file side in stored bytes and its dst_pitch in
-    result bytes.  Raises KeyError for a sliced name the file does not hold, ValueError for a malformed slice, a sliced name outside
-    `selected`, or a tensor load_file(dtype=...) cannot convert (see _cast_targets)."""
+    result bytes.  With `scales` ({float8 weight: name of its scale tensor}, dtype required; scale_block = (br, bc) for block scales)
+    every range gets one more item, the `scale` of Reader.readv_scaled_device with the scale tensor's NAME in place of its pointer: None,
+    or (scale name, scale_rows, scale_cols, block_rows, block_cols, cols, first_elem), first_elem being a sliced weight's offset in the
+    full tensor in elements.  Raises KeyError for a sliced name the file does not hold, ValueError for a malformed slice, a sliced name
+    outside `selected`, a tensor load_file(dtype=...) cannot convert (see _cast_targets) or a weight and scale load_file(scales=...)
+    cannot dequantize (see _scale_geometry)."""
     slices = dict(slices or {})
     sel = set(selected)
-    targets = _cast_targets(data_start, entries, selected, dtype) if dtype is not None else None
+    if scale_block is not None and scales is None:
+        raise ValueError("scale_block is given without scales")
+    geo = _scale_geometry(entries, selected, scales, scale_block, dtype) if scales is not None else None
+    targets = _cast_targets(data_start, entries, selected, dtype, geo or ()) if dtype is not None else None
     for name, spec in slices.items():
         if name not in entries:
             raise KeyError("the file holds no tensor named %r" % (name,))
@@ -166,6 +227,8 @@ def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=Non
         stored, shape, begin, end = entries[name]
         dt = targets[name] if targets is not None else stored
         tail = (stored, dt) if targets is not None else ()  # the dtypes of a readv_cast_device range
+        if geo is not None:  # and the scale of a readv_scaled_device range
+            tail += (geo[name] + (0,) if name in geo else None,)
         if name not in slices:
             out.append((name, dt, shape, (data_start + begin, end - begin, 1, 0, 0) + tail if end > begin else None))
             continue
@@ -179,6 +242,8 @@ def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=Non
             rows *= x
         row_len = (stop - start) * inner * stored.itemsize
         res = shape[:d] + (stop - start,) + shape[d + 1:]
+        if geo is not None and name in geo:  # the slice's first element in the full tensor
+            tail = tail[:-1] + (geo[name] + (start * inner,),)
         rng = (data_start + begin + start * inner * stored.itemsize, row_len, rows, shape[d] * inner * stored.itemsize,
                (stop - start) * inner * dt.itemsize) + tail if row_len and rows else None
         out.append((name, dt, res, rng))
@@ -186,16 +251,22 @@ def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=Non
 
 
 def load_file(fs: "_fs.CurvineFileSystem", path: str, device=None, names: Optional[Iterable[str]] = None,
-              verify: bool = True, slices: Optional[Dict[str, tuple]] = None, dtype=None) -> Dict[str, "object"]:
+              verify: bool = True, slices: Optional[Dict[str, tuple]] = None, dtype=None, scales: Optional[Dict[str, str]] = None,
+              scale_block: Optional[tuple] = None) -> Dict[str, "object"]:
     """The tensors of safetensors file `path` (all of them, or those in `names`) as tensors on `device` (default: the current CUDA
     device).  One vectored read moves them: blocks that no selected tensor touches are not fetched, and every touched block is
     CRC-verified whole, including the bytes of unselected neighbours that share it.  `slices` maps a name to (dim, start, stop): that
     tensor comes back contiguous with shape[dim] = stop - start -- a tensor-parallel rank's shard, without the rest of the tensor ever
     reaching HBM (see plan_ranges).  `dtype` (torch.float32, torch.float16 or torch.bfloat16) converts every float32, float16 and bfloat16
     tensor to it on the GPU in the same read, bit-identical to Tensor.to() on the CPU; integer and bool tensors come back as stored.  The
-    stored copy never exists in HBM: a converted tensor's blocks pass through the reader's bounded staging.  Raises IOError when a block
-    fails verification and `verify` is set, SafetensorsError for a malformed header, KeyError for a name the file does not hold,
-    ValueError for a malformed slice or a tensor `dtype` cannot convert (all before anything is allocated or read)."""
+    stored copy never exists in HBM: a converted tensor's blocks pass through the reader's bounded staging.  `scales` maps float8 weights
+    (F8_E4M3, F8_E5M2) to the names of their scale tensors in the same file (F32, F16 or BF16: one element, one per row of a 2-D weight,
+    or with scale_block = (br, bc) one per br x bc tile): those weights come back in `dtype`, dequantized on the GPU as they load, each
+    element (x.float() * scale.float()).to(dtype) bit for bit; they compose with `slices`.  The scales are read first, as stored, into
+    temporaries; the second read then dequantizes (two calls on the caller's stream, one verification).  Float8 tensors not named in
+    `scales` are refused, as without it.  Raises IOError when a block fails verification and `verify` is set, SafetensorsError for a
+    malformed header, KeyError for a name the file does not hold, ValueError for a malformed slice, a tensor `dtype` cannot convert or a
+    weight and scale that cannot be dequantized (all before anything is allocated or read)."""
     import torch
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     r, data_start, entries = _open_header(fs, path)
@@ -204,19 +275,32 @@ def load_file(fs: "_fs.CurvineFileSystem", path: str, device=None, names: Option
         for name in selected:
             if name not in entries:
                 raise KeyError("%s holds no tensor named %r" % (path, name))
-        plan = plan_ranges(data_start, entries, selected, slices, dtype)
+        plan = plan_ranges(data_start, entries, selected, slices, dtype, scales, scale_block)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        d_scales = {}  # scale name -> the scale tensor as stored, read by the first of the two calls
+        if scales is not None:
+            for sname in dict.fromkeys(rng[7][0] for _, _, _, rng in plan if rng is not None and rng[7] is not None):
+                sdt, sshape, begin, end = entries[sname]
+                d_scales[sname] = torch.empty((end - begin) // sdt.itemsize, dtype=sdt, device=dev)
+            r.readv_strided_device([(data_start + entries[n][2], entries[n][3] - entries[n][2], 1, 0, t.data_ptr(), 0)
+                                    for n, t in d_scales.items() if t.numel()], stream)
         out, ranges = {}, []
         for name, dt, shape, rng in plan:
             t = torch.empty(shape, dtype=dt, device=dev)
             out[name] = t
             if rng is not None:
                 file_off, row_len, rows, file_pitch, dst_pitch = rng[:5]
-                ranges.append((file_off, row_len, rows, file_pitch, t.data_ptr(), dst_pitch) + tuple(rng[5:]))
-        stream = torch.cuda.current_stream(dev).cuda_stream
+                tail = tuple(rng[5:])
+                if scales is not None and tail[2] is not None:  # the scale tensor's name -> its temporary
+                    sc = d_scales[tail[2][0]]
+                    tail = tail[:2] + ((sc.data_ptr(), sc.dtype) + tuple(tail[2][1:]),)
+                ranges.append((file_off, row_len, rows, file_pitch, t.data_ptr(), dst_pitch) + tail)
         if dtype is None:
             r.readv_strided_device(ranges, stream)
-        else:  # one call still: the ranges that convert nothing have src == dst, and their whole blocks land in place
+        elif scales is None:  # one call still: the ranges that convert nothing have src == dst, and their whole blocks land in place
             r.readv_cast_device(ranges, stream)
+        else:  # ordered after the scales' read on `stream`: each call waits for the stream at entry and makes it wait at exit
+            r.readv_scaled_device(ranges, stream)
         _, bad, _ = r.verify()
         if verify and bad:
             raise IOError("%d blocks of %s failed CRC verification" % (bad, path))

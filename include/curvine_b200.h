@@ -180,6 +180,31 @@ typedef struct CvCastRange {
     int32_t dst_dtype;
 } CvCastRange;          /* 56 bytes */
 int64_t cv_readv_cast_device(cv_reader* r, const CvCastRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes);
+/* Scaled device read: cv_readv_cast_device where a range may also carry the scales of an FP8 weight (FP8 checkpoints), dequantized on
+ * the GPU as they load: y = round_dst(f32(x) * f32(s)), one F32 multiply rounded once (cvk_gather_cast_scaled).  The weight is seen as a
+ * row-major 2-D view [V_rows, cols]; element e of range row k is view element first_elem + k * file_pitch + e (file_pitch in elements:
+ * an FP8 element is one byte), and view element (i, j) takes scale[(i / block_rows) * scale_cols + j / block_cols] from the
+ * scale_rows x scale_cols row-major buffer at d_scale.  Per-tensor scales are one element (block_rows = V_rows, block_cols = cols),
+ * per-row scales block_rows = 1, block_cols = cols; a tensor-parallel slice sets first_elem to its offset in the full tensor.
+ * d_scale == NULL: the range is a CvCastRange (FP8 sources are decoded exactly there too).  Plans exactly like cv_readv_cast_plan over
+ * the CvCastRange parts.  Errors besides those of cv_readv_cast_device (cv_last_error names the range): a scaled range whose source is
+ * not CV_DTYPE_F8_E4M3 / _E5M2 or whose destination is FP8; a scale dtype other than F32, F16, BF16; block_rows, block_cols, cols,
+ * scale_rows or scale_cols < 1, or first_elem < 0; scale_cols < ceil(cols / block_cols); the last view element the range touches in a
+ * scale row >= scale_rows; an int64 overflow in any of these; a scale buffer whose first or last byte is not device memory on the
+ * reader's device.  The scales must not change until the read is ordered on `stream`. */
+typedef struct CvScaledRange {
+    CvCastRange cast;
+    const void* d_scale;  /* NULL: not scaled */
+    int32_t scale_dtype;  /* CV_DTYPE_F32 / _F16 / _BF16 */
+    int32_t pad;
+    int64_t scale_rows;
+    int64_t scale_cols;
+    int64_t block_rows;
+    int64_t block_cols;
+    int64_t cols;         /* view columns: the weight's last dimension */
+    int64_t first_elem;   /* view element of the range's first element */
+} CvScaledRange;          /* 120 bytes */
+int64_t cv_readv_scaled_device(cv_reader* r, const CvScaledRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes);
 /* The plan cv_readv_cast_device executes, with the outputs of cv_readv_strided_plan (block_off and len in source bytes). */
 int64_t cv_readv_cast_plan(cv_reader* r, const CvCastRange* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len, int64_t* rows,
                            int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes);

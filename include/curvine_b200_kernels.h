@@ -18,6 +18,7 @@
  *                                                           curvine-fuse/src/session/fuse_response.rs:49-60,171-175
  *   cvk_gather_strided  (no reference counterpart: the rows of tensor-parallel slices of a checkpoint, strided reads)
  *   cvk_gather_cast     (no reference counterpart: checkpoint tensors converted to another float type on load)
+ *   cvk_gather_cast_scaled  (no reference counterpart: FP8 checkpoint weights dequantized with their scales on load)
  *   cvk_pack_frames     RpcMessage::encode_protocol +      orpc/src/message/rpc_message.rs:301-311,
  *                       RpcFrame::send/write_region          orpc/src/handler/rpc_frame.rs:97-121,205-220
  *                       (worker ReadHandler::read response)  curvine-server/src/worker/handler/read_handler.rs:143-183
@@ -110,11 +111,15 @@ typedef struct CvStridedSeg {
     uint64_t dst_pitch;
 } CvStridedSeg;
 
-/* element types of cvk_gather_cast and of cast reads (CvCastRange).  CV_DTYPE_NONE: bytes as stored, no conversion. */
+/* element types of cvk_gather_cast and of cast reads (CvCastRange).  CV_DTYPE_NONE: bytes as stored, no conversion.  The two FP8
+ * codes are source types only, converted by cvk_gather_cast_scaled: E4M3 is torch's float8_e4m3fn (no infinities, 0x7f / 0xff are
+ * NaN), E5M2 is float8_e5m2. */
 #define CV_DTYPE_NONE 0
 #define CV_DTYPE_F32 1
 #define CV_DTYPE_F16 2
 #define CV_DTYPE_BF16 3
+#define CV_DTYPE_F8_E4M3 4
+#define CV_DTYPE_F8_E5M2 5
 
 /* Work chunks of one row of `elems` elements in cvk_gather_cast: a chunk is 8 elements whose destination starts 16-byte aligned, plus
  * a head chunk for the elements in front of the first aligned one. */
@@ -134,6 +139,22 @@ typedef struct CvCastSeg {
     int32_t src_dtype;   /* CV_DTYPE_F32 / _F16 / _BF16 */
     int32_t dst_dtype;
 } CvCastSeg;             /* 64 bytes */
+
+/* scale of a cast segment in cvk_gather_cast_scaled (one per CvCastSeg, same index).  The segment's elements are elements of a
+ * weight seen as a row-major 2-D view [V_rows, cols]: element e of segment row k is view element view0 + k*view_step + e, and view
+ * element (i, j) is multiplied by scale[(i / block_rows) * scale_cols + j / block_cols] before it is rounded to the destination.
+ * scale == NULL: the segment is not scaled. */
+typedef struct CvScaleSeg {
+    const void* scale;   /* scale elements in HBM, row-major */
+    uint64_t block_rows; /* view rows per scale row */
+    uint64_t block_cols; /* view columns per scale column */
+    uint64_t scale_cols;
+    uint64_t cols;       /* view columns */
+    uint64_t view0;      /* view element of the segment's row 0, element 0 */
+    uint64_t view_step;  /* view elements between the starts of two segment rows */
+    int32_t scale_dtype; /* CV_DTYPE_F32 / _F16 / _BF16 */
+    int32_t pad;
+} CvScaleSeg;            /* 64 bytes */
 
 /* Build the per-device constant tables (both polynomials).  Optional: every launcher does it lazily. */
 int cvk_init(int device);
@@ -185,6 +206,17 @@ int cvk_gather_strided(const uint8_t* d_src, const CvStridedSeg* d_segs, uint32_
  * total_elems = sum of elems * rows (sizes the grid; 0 launches nothing).  Rows of different segments must not overlap in d_dst.
  * Algorithmic bytes: reads N * src size, writes N * dst size. */
 int cvk_gather_cast(const uint8_t* d_src, const CvCastSeg* d_segs, uint32_t n, uint64_t total_elems, uint8_t* d_dst, cv_stream_t stream);
+
+/* K5, scaled instance: cvk_gather_cast with FP8 sources (CV_DTYPE_F8_E4M3 / _E5M2, decoded exactly) and a scale per element.
+ * d_scales[i] belongs to d_segs[i].  A segment with a scale gives y = round_dst(f32(x) * f32(s)): one IEEE F32 multiply (never
+ * contracted, denormals kept), rounded once to dst_dtype as in cvk_gather_cast -- bit-identical to torch's CPU
+ * (x.float() * s.float()).to(dst) for every non-NaN result.  A segment without one converts as cvk_gather_cast does (FP8 exactly).
+ * The scale of an element is found from its view position once per 8-element chunk and stepped from there; the scale element index
+ * must lie inside the caller's scale buffer (cv_readv_scaled_device validates it).  FP8 sources need no alignment; whole chunks read
+ * them in one 8-byte load when it is aligned.  d_scales may be NULL only when n == 0.  Algorithmic bytes: reads N * src size plus
+ * the scales, writes N * dst size. */
+int cvk_gather_cast_scaled(const uint8_t* d_src, const CvCastSeg* d_segs, const CvScaleSeg* d_scales, uint32_t n, uint64_t total_elems,
+                           uint8_t* d_dst, cv_stream_t stream);
 
 /* K4: worker-side inverse of K2.  For frame f: write the 22-byte prefix (+ no header) at
  * d_wire + d_desc[f].wire_off, copy d_src[dst_off .. +data_len) behind it, and CRC the source bytes
