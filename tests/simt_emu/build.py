@@ -174,13 +174,30 @@ def _digest(extra):
 
 
 MUTATIONS = {
-    # planted bugs for the checks that are supposed to find them (tools/sanitize_ingest.sh): name -> (file under csrc/host, old text, new text)
-    "copies_do_not_wait_for_the_callers_stream": ("gpu_reader.cu", "for (auto cs : G.copy_streams) CU_TRY(cudaStreamWaitEvent(cs, G.entry_ev, 0));",
+    # planted bugs for the checks that are supposed to find them (tools/sanitize_ingest.sh, tests/test_launch_shapes_mutants.py):
+    # name -> (file under csrc/, old text, new text)
+    "copies_do_not_wait_for_the_callers_stream": ("host/gpu_reader.cu", "for (auto cs : G.copy_streams) CU_TRY(cudaStreamWaitEvent(cs, G.entry_ev, 0));",
                                                    "/* planted: the copy streams start without waiting for what the caller enqueued before the read */;"),
-    "callers_stream_does_not_wait_for_the_read": ("gpu_reader.cu", "CU_TRY(cudaStreamWaitEvent(static_cast<cudaStream_t>(user_stream), G.done_ev, 0));",
+    "callers_stream_does_not_wait_for_the_read": ("host/gpu_reader.cu", "CU_TRY(cudaStreamWaitEvent(static_cast<cudaStream_t>(user_stream), G.done_ev, 0));",
                                                    "/* planted: the caller's stream continues without waiting for the read */;"),
-    "verifier_does_not_wait_for_the_copy": ("gpu_reader.cu", "cudaStreamWaitEvent(G.vstream, G.copy_ev[g % NS], 0);", "/* planted: the verify stream no longer waits for the group's copies */;"),
+    "verifier_does_not_wait_for_the_copy": ("host/gpu_reader.cu", "cudaStreamWaitEvent(G.vstream, G.copy_ev[g % NS], 0);", "/* planted: the verify stream no longer waits for the group's copies */;"),
+    # K5's scale walk divides view positions in 32 bits even when a position or the view's width is >= 2^32
+    "scale_walk_divides_in_32_bits": ("kernels.cu", "{ return (a | b) >> 32 ? a / b : uint64_t(uint32_t(a) / uint32_t(b)); }",
+                                      "{ return uint64_t(uint32_t(a) / uint32_t(b)); /* planted: always 32-bit */ }"),
+    # the shifted walk loses its row count above 1023 rows of 512 bytes: wrong only for segments of >= 512 KiB (s >= 19)
+    "shifted_walk_drops_rows_past_1023": ("kernels.cu", "const uint32_t R = L >> 9, nv = (L & 511u) >> 4;\n    const uint32_t nvec = (L >> 4) + 1;",
+                                          "const uint32_t R = (L >> 9) & 0x3ffu, nv = (L & 511u) >> 4;  /* planted */\n    const uint32_t nvec = (L >> 4) + 1;"),
 }
+
+
+def _mutated(fname, text, mutate):
+    """text of csrc/<fname>, with the planted bug `mutate` in it if that bug lives in this file"""
+    if not mutate or MUTATIONS[mutate][0] != fname:
+        return text
+    _, old, new = MUTATIONS[mutate]
+    if text.count(old) != 1:
+        raise RuntimeError("mutation %s: the text to replace occurs %d times in %s" % (mutate, text.count(old), fname))
+    return text.replace(old, new)
 
 
 def build(sanitize: str = "", mutate: str = "") -> str:
@@ -191,7 +208,7 @@ def build(sanitize: str = "", mutate: str = "") -> str:
         return lib
     os.makedirs(out_dir, exist_ok=True)
     kern = os.path.join(out_dir, "kernels_rewritten.cc")
-    text = rewrite(open(os.path.join(CSRC, "kernels.cu")).read())
+    text = rewrite(_mutated("kernels.cu", open(os.path.join(CSRC, "kernels.cu")).read(), mutate))
     # the rewritten copy sits in /tmp: its two relative includes are made absolute
     text = text.replace('#include "../../include/curvine_b200_kernels.h"', '#include "%s"' % os.path.join(ROOT, "include", "curvine_b200_kernels.h"))
     text = text.replace('#include "crc_gf.h"', '#include "%s"' % os.path.join(CSRC, "crc_gf.h"))
@@ -200,16 +217,13 @@ def build(sanitize: str = "", mutate: str = "") -> str:
     san = ["-fsanitize=" + sanitize, "-fno-omit-frame-pointer"] if sanitize else []
     jobs = []
     srcs = sources()
-    if mutate:
-        fname, old, new = MUTATIONS[mutate]
-        text = open(os.path.join(HOST, fname)).read()
-        if text.count(old) != 1:
-            raise RuntimeError("mutation %s: the text to replace occurs %d times in %s" % (mutate, text.count(old), fname))
-        os.makedirs(out_dir, exist_ok=True)
-        mutated = os.path.join(out_dir, "mutated_" + fname)
+    if mutate and MUTATIONS[mutate][0].startswith("host/"):
+        fname = MUTATIONS[mutate][0]
+        name = os.path.basename(fname)
+        mutated = os.path.join(out_dir, "mutated_" + name)
         with open(mutated, "w") as f:  # its relative includes resolve through -I HOST below
-            f.write(text.replace(old, new))
-        srcs = [mutated if os.path.basename(x) == fname else x for x in srcs]
+            f.write(_mutated(fname, open(os.path.join(CSRC, fname)).read(), mutate))
+        srcs = [mutated if os.path.basename(x) == name else x for x in srcs]
     for src in srcs:
         extra = ["-O1", "-I", MOCK] + san
         if sanitize == "thread" and os.path.basename(src) == "simt_emu.cc":
