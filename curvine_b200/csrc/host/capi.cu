@@ -80,6 +80,75 @@ struct cv_worker {
     std::string hostname;
 };
 
+static Err ensure_dev(cv_reader* r) {
+    if (r->dev) return Err::ok();
+    return GpuFsReader::open(r->ctx.get(), r->path, &r->dev);
+}
+
+// One ReadvRange per ABI range: a plain range is a strided range of one row, a cast range a strided range with dtypes, a scaled range
+// a cast range with a scale.
+static ReadvRange to_readv(const CvRange& s) { return ReadvRange{s.file_off, s.len, static_cast<uint8_t*>(s.d_dst)}; }
+
+static ReadvRange to_readv(const CvStridedRange& s) {
+    return ReadvRange{s.file_off, s.row_len, static_cast<uint8_t*>(s.d_dst), s.rows, s.file_pitch, s.dst_pitch};
+}
+
+static ReadvRange to_readv(const CvCastRange& s) {
+    return ReadvRange{s.file_off, s.row_len, static_cast<uint8_t*>(s.d_dst), s.rows, s.file_pitch, s.dst_pitch, s.src_dtype, s.dst_dtype};
+}
+
+static ReadvRange to_readv(const CvScaledRange& s) {
+    ReadvRange r = to_readv(s.cast);
+    r.scale = ReadvScale{s.d_scale, s.scale_dtype, s.scale_rows, s.scale_cols, s.block_rows, s.block_cols, s.cols, s.first_elem};
+    return r;
+}
+
+template <typename Range>
+static std::vector<ReadvRange> to_readv(const Range* ranges, int32_t n) {
+    std::vector<ReadvRange> out;
+    for (int32_t i = 0; ranges && i < n; i++) out.push_back(to_readv(ranges[i]));
+    return out;
+}
+
+template <typename Range>
+static int64_t readv_device_body(cv_reader* r, const Range* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes) {
+    API_TRY(ensure_dev(r));
+    const std::vector<ReadvRange> rs = to_readv(ranges, n);
+    int64_t got = 0;
+    API_TRY(r->dev->readv_device(rs.data(), n, stream, &got));
+    *nbytes = got;
+    return ok();
+}
+
+// The plan's spans into the caller's arrays (any of which may be NULL); `rows` only for the strided form.
+template <typename Range>
+static int64_t readv_plan_body(cv_reader* r, const Range* ranges, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len, int64_t* rows,
+                               int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes) {
+    const FileBlocks& fb = r->host->file_blocks();
+    const std::vector<ReadvRange> rs = to_readv(ranges, n);
+    std::vector<ReadvBlock> blocks;
+    std::vector<ReadvSpan> spans;
+    API_TRY(plan_readv(fb, rs.data(), n, &blocks, &spans));
+    int64_t fetched = 0;
+    size_t i = 0;
+    for (const ReadvBlock& b : blocks) {
+        fetched += fb.block_locs[b.block].block.len;
+        for (size_t k = b.first_span; k < b.first_span + b.n_spans; k++, i++) {
+            if (i >= static_cast<size_t>(std::max(cap, 0))) continue;
+            if (block_index) block_index[i] = static_cast<int64_t>(b.block);
+            if (block_off) block_off[i] = spans[k].block_off;
+            if (len) len[i] = spans[k].len;
+            if (rows) rows[i] = spans[k].rows;
+            if (range_index) range_index[i] = spans[k].range;
+            if (direct) direct[i] = b.direct ? 1 : 0;
+        }
+    }
+    if (n_spans) *n_spans = static_cast<int32_t>(spans.size());
+    if (n_blocks) *n_blocks = static_cast<int64_t>(blocks.size());
+    if (fetch_bytes) *fetch_bytes = fetched;
+    return ok();
+}
+
 extern "C" {
 
 const char* cv_last_error(void) { return g_last_error.c_str(); }
@@ -266,11 +335,6 @@ int64_t cv_close_reader(cv_reader* r) {
     API_GUARD_END
 }
 
-static Err ensure_dev(cv_reader* r) {
-    if (r->dev) return Err::ok();
-    return GpuFsReader::open(r->ctx.get(), r->path, &r->dev);
-}
-
 int64_t cv_read_device(cv_reader* r, void* d_dst, int64_t cap, cv_stream_t stream, int64_t* nbytes) {
     API_GUARD_BEGIN
     API_NEED(r);
@@ -337,83 +401,12 @@ int64_t cv_shard_plan(cv_reader* r, int32_t rank, int32_t world, int64_t* block_
     API_GUARD_END
 }
 
-// a plain range is a strided range of one row
-static std::vector<ReadvRange> readv_ranges(const CvRange* ranges, int32_t n) {
-    std::vector<ReadvRange> out;
-    for (int32_t i = 0; ranges && i < n; i++) out.push_back(ReadvRange{ranges[i].file_off, ranges[i].len, static_cast<uint8_t*>(ranges[i].d_dst)});
-    return out;
-}
-
-static std::vector<ReadvRange> strided_ranges(const CvStridedRange* ranges, int32_t n) {
-    std::vector<ReadvRange> out;
-    for (int32_t i = 0; ranges && i < n; i++) {
-        const CvStridedRange& s = ranges[i];
-        out.push_back(ReadvRange{s.file_off, s.row_len, static_cast<uint8_t*>(s.d_dst), s.rows, s.file_pitch, s.dst_pitch});
-    }
-    return out;
-}
-
-static std::vector<ReadvRange> cast_ranges(const CvCastRange* ranges, int32_t n) {
-    std::vector<ReadvRange> out;
-    for (int32_t i = 0; ranges && i < n; i++) {
-        const CvCastRange& s = ranges[i];
-        out.push_back(ReadvRange{s.file_off, s.row_len, static_cast<uint8_t*>(s.d_dst), s.rows, s.file_pitch, s.dst_pitch, s.src_dtype, s.dst_dtype});
-    }
-    return out;
-}
-
-static std::vector<ReadvRange> scaled_ranges(const CvScaledRange* ranges, int32_t n) {
-    std::vector<ReadvRange> out;
-    for (int32_t i = 0; ranges && i < n; i++) {
-        const CvScaledRange& s = ranges[i];
-        const CvCastRange& c = s.cast;
-        out.push_back(ReadvRange{c.file_off, c.row_len, static_cast<uint8_t*>(c.d_dst), c.rows, c.file_pitch, c.dst_pitch, c.src_dtype, c.dst_dtype,
-                                 ReadvScale{s.d_scale, s.scale_dtype, s.scale_rows, s.scale_cols, s.block_rows, s.block_cols, s.cols, s.first_elem}});
-    }
-    return out;
-}
-
-static int64_t readv_device_common(cv_reader* r, const std::vector<ReadvRange>& rs, int32_t n, cv_stream_t stream, int64_t* nbytes) {
-    API_TRY(ensure_dev(r));
-    int64_t got = 0;
-    API_TRY(r->dev->readv_device(rs.data(), n, stream, &got));
-    *nbytes = got;
-    return ok();
-}
-
-// The plan's spans into the caller's arrays (any of which may be NULL); `rows` only for the strided form.
-static int64_t readv_plan_common(cv_reader* r, const std::vector<ReadvRange>& rs, int32_t n, int64_t* block_index, int64_t* block_off, int64_t* len,
-                                 int64_t* rows, int32_t* range_index, int32_t* direct, int32_t cap, int32_t* n_spans, int64_t* n_blocks, int64_t* fetch_bytes) {
-    const FileBlocks& fb = r->host->file_blocks();
-    std::vector<ReadvBlock> blocks;
-    std::vector<ReadvSpan> spans;
-    API_TRY(plan_readv(fb, rs.data(), n, &blocks, &spans));
-    int64_t fetched = 0;
-    size_t i = 0;
-    for (const ReadvBlock& b : blocks) {
-        fetched += fb.block_locs[b.block].block.len;
-        for (size_t k = b.first_span; k < b.first_span + b.n_spans; k++, i++) {
-            if (i >= static_cast<size_t>(std::max(cap, 0))) continue;
-            if (block_index) block_index[i] = static_cast<int64_t>(b.block);
-            if (block_off) block_off[i] = spans[k].block_off;
-            if (len) len[i] = spans[k].len;
-            if (rows) rows[i] = spans[k].rows;
-            if (range_index) range_index[i] = spans[k].range;
-            if (direct) direct[i] = b.direct ? 1 : 0;
-        }
-    }
-    if (n_spans) *n_spans = static_cast<int32_t>(spans.size());
-    if (n_blocks) *n_blocks = static_cast<int64_t>(blocks.size());
-    if (fetch_bytes) *fetch_bytes = fetched;
-    return ok();
-}
-
 int64_t cv_readv_device(cv_reader* r, const CvRange* ranges, int32_t n, cv_stream_t stream, int64_t* nbytes) {
     API_GUARD_BEGIN
     API_NEED(r);
     API_NEED(nbytes);
     if (n > 0) API_NEED(ranges);
-    return readv_device_common(r, readv_ranges(ranges, n), n, stream, nbytes);
+    return readv_device_body(r, ranges, n, stream, nbytes);
     API_GUARD_END
 }
 
@@ -422,8 +415,7 @@ int64_t cv_readv_plan(cv_reader* r, const CvRange* ranges, int32_t n, int64_t* b
     API_GUARD_BEGIN
     API_NEED(r);
     if (n > 0) API_NEED(ranges);
-    return readv_plan_common(r, readv_ranges(ranges, n), n, block_index, block_off, len, nullptr, range_index, direct, cap, n_spans, n_blocks,
-                             fetch_bytes);
+    return readv_plan_body(r, ranges, n, block_index, block_off, len, nullptr, range_index, direct, cap, n_spans, n_blocks, fetch_bytes);
     API_GUARD_END
 }
 
@@ -432,7 +424,7 @@ int64_t cv_readv_strided_device(cv_reader* r, const CvStridedRange* ranges, int3
     API_NEED(r);
     API_NEED(nbytes);
     if (n > 0) API_NEED(ranges);
-    return readv_device_common(r, strided_ranges(ranges, n), n, stream, nbytes);
+    return readv_device_body(r, ranges, n, stream, nbytes);
     API_GUARD_END
 }
 
@@ -441,7 +433,7 @@ int64_t cv_readv_strided_plan(cv_reader* r, const CvStridedRange* ranges, int32_
     API_GUARD_BEGIN
     API_NEED(r);
     if (n > 0) API_NEED(ranges);
-    return readv_plan_common(r, strided_ranges(ranges, n), n, block_index, block_off, len, rows, range_index, direct, cap, n_spans, n_blocks, fetch_bytes);
+    return readv_plan_body(r, ranges, n, block_index, block_off, len, rows, range_index, direct, cap, n_spans, n_blocks, fetch_bytes);
     API_GUARD_END
 }
 
@@ -450,7 +442,7 @@ int64_t cv_readv_cast_device(cv_reader* r, const CvCastRange* ranges, int32_t n,
     API_NEED(r);
     API_NEED(nbytes);
     if (n > 0) API_NEED(ranges);
-    return readv_device_common(r, cast_ranges(ranges, n), n, stream, nbytes);
+    return readv_device_body(r, ranges, n, stream, nbytes);
     API_GUARD_END
 }
 
@@ -459,7 +451,7 @@ int64_t cv_readv_scaled_device(cv_reader* r, const CvScaledRange* ranges, int32_
     API_NEED(r);
     API_NEED(nbytes);
     if (n > 0) API_NEED(ranges);
-    return readv_device_common(r, scaled_ranges(ranges, n), n, stream, nbytes);
+    return readv_device_body(r, ranges, n, stream, nbytes);
     API_GUARD_END
 }
 
@@ -468,7 +460,7 @@ int64_t cv_readv_cast_plan(cv_reader* r, const CvCastRange* ranges, int32_t n, i
     API_GUARD_BEGIN
     API_NEED(r);
     if (n > 0) API_NEED(ranges);
-    return readv_plan_common(r, cast_ranges(ranges, n), n, block_index, block_off, len, rows, range_index, direct, cap, n_spans, n_blocks, fetch_bytes);
+    return readv_plan_body(r, ranges, n, block_index, block_off, len, rows, range_index, direct, cap, n_spans, n_blocks, fetch_bytes);
     API_GUARD_END
 }
 
@@ -942,23 +934,6 @@ int64_t cv_synth_create_file(cv_worker* w, const char* path, int64_t inode_id, i
     }
     return ok();
     API_GUARD_END
-}
-
-// The host sources are also linked without csrc/kernels.cu (the host-only test library of tests/mock_cuda, whose CPU stand-ins cover the
-// launchers that existed before this one).  There this weak definition keeps the symbol resolvable and reports the strided gather as
-// unsupported; it copies nothing.  Every library that links kernels.cu gets the kernel: the strong definition there replaces this one.
-__attribute__((weak)) int cvk_gather_strided(const uint8_t*, const CvStridedSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) {
-    return n ? int(cudaErrorNotSupported) : 0;
-}
-
-// The same for the cast gather of cast reads (cv_readv_cast_device).
-__attribute__((weak)) int cvk_gather_cast(const uint8_t*, const CvCastSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) {
-    return n ? int(cudaErrorNotSupported) : 0;
-}
-
-// And for K5's scaled instance (FP8 sources and scales of cv_readv_scaled_device / cv_readv_cast_device).
-__attribute__((weak)) int cvk_gather_cast_scaled(const uint8_t*, const CvCastSeg*, const CvScaleSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) {
-    return n ? int(cudaErrorNotSupported) : 0;
 }
 
 }  // extern "C"

@@ -7,6 +7,7 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <array>
 #include <fstream>
 
 #include "../../../include/curvine_b200_kernels.h"
@@ -288,6 +289,88 @@ Err GpuFsReader::complete() {
     return verify(&s, &b, &v);
 }
 
+static bool is_f8(int32_t dt) { return dt == CV_DTYPE_F8_E4M3 || dt == CV_DTYPE_F8_E5M2; }
+static int64_t dtype_size(int32_t dt) { return dt == CV_DTYPE_F32 ? 4 : dt == CV_DTYPE_NONE || is_f8(dt) ? 1 : 2; }
+
+// every table of the per-call table image starts 256-byte aligned
+static size_t table_up(size_t x) { return (x + 255) & ~size_t(255); }
+
+// Delivery riding on a read: after the bytes landed in d_dst and were CRC'd, spans of them are copied or converted to d_out + dst_off,
+// in the same launch train on the verify stream, no extra sync.  Page buffers of a FUSE reply (Reader::fuse_read +
+// ResponseData::as_iovec on the device), or the spans of the boundary blocks of a vectored read: one-row spans as segs (K3), spans of
+// several rows as strided (K3 over 2D descriptors), spans of converting ranges as casts (K5).  When a cast span has an FP8 source or a
+// scale, `scales` (one CvScaleSeg per cast, a null scale for the others) is uploaded too and K5's scaled instance runs instead of K5.
+struct GpuFsReader::Scatter {
+    uint8_t* d_out;
+    std::vector<CvSeg> segs;
+    uint64_t total = 0;  // sum of segs[i].len
+    std::vector<CvStridedSeg> strided;
+    uint64_t strided_total = 0;  // sum of strided[i].len * strided[i].rows
+    std::vector<CvCastSeg> casts;
+    uint64_t cast_elems = 0, cast_chunks = 0;  // sum of casts[i].elems * rows, and the next segment's `first`
+    std::vector<CvScaleSeg> scales;
+    bool scaled = false;  // a cast span has an FP8 source or a scale
+
+    explicit Scatter(uint8_t* out) : d_out(out) {}
+
+    // A span of range `r`: row k < rows is `len` source bytes at d_dst + src + k * file_pitch, delivered to d_out + dst + k * dst_pitch
+    // (converted when the range converts).  `file_pos` is the file offset of the span's first byte.
+    void add(uint64_t src, uint64_t dst, uint64_t len, uint64_t rows, const ReadvRange& r, int64_t file_pos) {
+        if (r.cast()) {
+            const int64_t ss = dtype_size(r.src_dtype);
+            const uint64_t elems = len / static_cast<uint64_t>(ss);
+            casts.push_back(CvCastSeg{src, dst, elems, rows, static_cast<uint64_t>(r.file_pitch), static_cast<uint64_t>(r.dst_pitch), cast_chunks,
+                                      r.src_dtype, r.dst_dtype});
+            cast_elems += elems * rows;
+            cast_chunks += rows * CV_CAST_ROW_CHUNKS(elems);
+            // the view position of the span's first element: first_elem + (its file offset - file_off) / src size
+            const ReadvScale& g = r.scale;
+            scales.push_back(r.scaled() ? CvScaleSeg{g.ptr, uint64_t(g.block_rows), uint64_t(g.block_cols), uint64_t(g.cols), uint64_t(g.view_cols),
+                                                     uint64_t(g.first_elem + (file_pos - r.file_off) / ss), uint64_t(r.file_pitch / ss), g.dtype, 0}
+                                        : CvScaleSeg{});
+            scaled |= r.scaled() || is_f8(r.src_dtype);
+        } else if (rows == 1) {
+            segs.push_back(CvSeg{src, dst, len});
+            total += len;
+        } else {
+            strided.push_back(CvStridedSeg{src, dst, len, rows, static_cast<uint64_t>(r.file_pitch), static_cast<uint64_t>(r.dst_pitch)});
+            strided_total += len * rows;
+        }
+    }
+
+    // The scatter's section of the per-call tables: segs | strided | casts | scales (when scaled).  [k] = where table k starts, [4] = bytes.
+    std::array<size_t, 5> offsets() const {
+        std::array<size_t, 5> o{};
+        o[1] = table_up(sizeof(CvSeg) * segs.size());
+        o[2] = o[1] + table_up(sizeof(CvStridedSeg) * strided.size());
+        o[3] = o[2] + table_up(sizeof(CvCastSeg) * casts.size());
+        o[4] = o[3] + (scaled ? table_up(sizeof(CvScaleSeg) * scales.size()) : 0);
+        return o;
+    }
+    size_t bytes() const { return offsets()[4]; }
+    template <typename T>
+    T* table(uint8_t* section, int k) const { return reinterpret_cast<T*>(section + offsets()[k]); }
+
+    // the tables into the section's pinned image
+    void write(uint8_t* h) const {
+        std::copy(segs.begin(), segs.end(), table<CvSeg>(h, 0));
+        std::copy(strided.begin(), strided.end(), table<CvStridedSeg>(h, 1));
+        std::copy(casts.begin(), casts.end(), table<CvCastSeg>(h, 2));
+        if (scaled) std::copy(scales.begin(), scales.end(), table<CvScaleSeg>(h, 3));
+    }
+
+    // K3, K3 over 2D descriptors, then K5 or its scaled instance, out of d_src with the tables uploaded at d; a kind without spans
+    // launches nothing
+    Err launch(const uint8_t* d_src, uint8_t* d, cudaStream_t s) const {
+        if (!segs.empty()) CVK_TRY(cvk_gather_pages(d_src, table<CvSeg>(d, 0), static_cast<uint32_t>(segs.size()), total, d_out, s));
+        if (!strided.empty()) CVK_TRY(cvk_gather_strided(d_src, table<CvStridedSeg>(d, 1), static_cast<uint32_t>(strided.size()), strided_total, d_out, s));
+        const uint32_t n_casts = static_cast<uint32_t>(casts.size());
+        if (n_casts && scaled) CVK_TRY(cvk_gather_cast_scaled(d_src, table<CvCastSeg>(d, 2), table<CvScaleSeg>(d, 3), n_casts, cast_elems, d_out, s));
+        else if (n_casts) CVK_TRY(cvk_gather_cast(d_src, table<CvCastSeg>(d, 2), n_casts, cast_elems, d_out, s));
+        return Err::ok();
+    }
+};
+
 Err GpuFsReader::fuse_read_device(int64_t want, void* d_scratch, void* d_page_base, const uint64_t* page_offsets, int64_t n_pages, int64_t page_size,
                                    void* stream, int64_t* n) {
     *n = 0;
@@ -295,16 +378,16 @@ Err GpuFsReader::fuse_read_device(int64_t want, void* d_scratch, void* d_page_ba
     const int64_t take = std::max<int64_t>(0, std::min(want, len() - pos_));
     const int64_t need_pages = (take + page_size - 1) / page_size;
     if (need_pages > n_pages) return Err::common("not enough page buffers for the reply");
-    Scatter ps;
-    ps.d_out = static_cast<uint8_t*>(d_page_base), ps.total = static_cast<uint64_t>(take);
+    Scatter ps(static_cast<uint8_t*>(d_page_base));
+    const ReadvRange bytes{};  // a page is one row of a plain byte range
     for (int64_t i = 0; i < need_pages; i++)
-        ps.segs.push_back(CvSeg{static_cast<uint64_t>(i * page_size), page_offsets[i], static_cast<uint64_t>(std::min(page_size, take - i * page_size))});
-    return read_device_impl(d_scratch, take, stream, n, need_pages > 0 ? &ps : nullptr);
+        ps.add(static_cast<uint64_t>(i * page_size), page_offsets[i], static_cast<uint64_t>(std::min(page_size, take - i * page_size)), 1, bytes, 0);
+    return read_device_impl(d_scratch, take, stream, n, &ps);
 }
 
 Err GpuFsReader::read_device(void* d_dst, int64_t cap, void* stream, int64_t* n) { return read_device_impl(d_dst, cap, stream, n, nullptr); }
 
-Err GpuFsReader::read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const Scatter* pages) {
+Err GpuFsReader::read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const Scatter* scatter) {
     *n = 0;
     const int64_t end = std::min(len(), pos_ + std::max<int64_t>(cap, 0));
     if (end <= pos_) return Err::ok();
@@ -319,7 +402,7 @@ Err GpuFsReader::read_device_impl(void* d_dst, int64_t cap, void* stream, int64_
         jobs.push_back(Job{&(*fbp_).block_locs[idx], boff, take, p - pos_, boff == 0 && take == blen});
         p += take;
     }
-    CV_RETURN_IF_ERR(run_jobs(jobs, static_cast<uint8_t*>(d_dst), stream, pages));
+    CV_RETURN_IF_ERR(run_jobs(jobs, static_cast<uint8_t*>(d_dst), stream, scatter));
     *n = end - pos_;
     pos_ = end;
     return Err::ok();
@@ -350,9 +433,6 @@ Err GpuFsReader::read_device_sharded(int rank, int world, void* d_dst, int64_t c
     *n = total;
     return Err::ok();
 }
-
-static bool is_f8(int32_t dt) { return dt == CV_DTYPE_F8_E4M3 || dt == CV_DTYPE_F8_E5M2; }
-static int64_t dtype_size(int32_t dt) { return dt == CV_DTYPE_F32 ? 4 : dt == CV_DTYPE_NONE || is_f8(dt) ? 1 : 2; }
 
 // A range's destination row in bytes: row_len converted to the destination element size.
 static int64_t dst_row_len(const ReadvRange& r) { return r.cast() ? r.row_len / dtype_size(r.src_dtype) * dtype_size(r.dst_dtype) : r.row_len; }
@@ -658,34 +738,27 @@ static Err check_device_dst(const void* p, int device) {
 enum JobMode : uint8_t { kPlain = 0, kFramed = 1, kHole = 3 };
 
 // Layout of the per-call device tables (shared by all readers of the context) and of their pinned host image:
-//   off[J] len[J] expect[J] skip[J] | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F] | segs[n_segs] | strided[n_strided] | casts[n_casts]
-//   | scales[n_scales]
-// off .. skip are uploaded before the fetch starts; crc .. ferr are the results copied back.
+//   off[J] len[J] expect[J] skip[J] | scatter section | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F]
+// off .. the scatter section are uploaded in one copy before the fetch starts; crc .. ferr are the results copied back.
 struct TableLayout {
-    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, o_segs = 0, o_strided = 0, o_casts = 0, o_scales = 0, bytes = 0;
+    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_scatter = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, bytes = 0;
     TableLayout() = default;
-    TableLayout(size_t j, size_t f, size_t n_segs, size_t n_strided, size_t n_casts, size_t n_scales) : J(j), F(f) {
-        auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
-        o_len = up(8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_crc = up(o_skip + J);
+    TableLayout(size_t j, size_t f, size_t scatter_bytes) : J(j), F(f) {
+        const auto up = table_up;
+        o_len = up(8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_scatter = up(o_skip + J), o_crc = up(o_scatter + scatter_bytes);
         o_streams = up(o_crc + 4 * res_words()), o_fdesc = up(o_streams + sizeof(CvStreamDesc) * J);
-        o_segs = up(o_fdesc + sizeof(CvFrameDesc) * F), o_strided = up(o_segs + sizeof(CvSeg) * n_segs);
-        o_casts = up(o_strided + sizeof(CvStridedSeg) * n_strided);
-        o_scales = up(o_casts + sizeof(CvCastSeg) * n_casts);
-        bytes = up(o_scales + sizeof(CvScaleSeg) * n_scales);
+        bytes = up(o_fdesc + sizeof(CvFrameDesc) * F);
     }
     size_t res_words() const { return J + 4 + F; }
     uint64_t* off(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t); }
     uint64_t* len(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t + o_len); }
     uint32_t* expect(uint8_t* t) const { return reinterpret_cast<uint32_t*>(t + o_exp); }
     uint8_t* skip(uint8_t* t) const { return t + o_skip; }
+    uint8_t* scatter(uint8_t* t) const { return t + o_scatter; }
     uint32_t* crc(uint8_t* t) const { return reinterpret_cast<uint32_t*>(t + o_crc); }
     uint32_t* ferr(uint8_t* t) const { return crc(t) + J + 4; }
     CvStreamDesc* streams(uint8_t* t) const { return reinterpret_cast<CvStreamDesc*>(t + o_streams); }
     CvFrameDesc* fdesc(uint8_t* t) const { return reinterpret_cast<CvFrameDesc*>(t + o_fdesc); }
-    CvSeg* segs(uint8_t* t) const { return reinterpret_cast<CvSeg*>(t + o_segs); }
-    CvStridedSeg* strided(uint8_t* t) const { return reinterpret_cast<CvStridedSeg*>(t + o_strided); }
-    CvCastSeg* casts(uint8_t* t) const { return reinterpret_cast<CvCastSeg*>(t + o_casts); }
-    CvScaleSeg* scales(uint8_t* t) const { return reinterpret_cast<CvScaleSeg*>(t + o_scales); }
 };
 
 // What one run_jobs call does, decided before any CUDA call.
@@ -705,7 +778,7 @@ struct GpuFsReader::CallPlan {
     TableLayout tl;
 };
 
-Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, size_t n_casts, size_t n_scales, CallPlan* out) const {
+Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t scatter_bytes, CallPlan* out) const {
     CallPlan& P = *out;
     const B200Conf& bc = ctx_->conf.b200;
     const size_t J = jobs.size();
@@ -751,7 +824,7 @@ Err GpuFsReader::plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n
     P.group_verbatim.assign(P.NG, 0);
     for (size_t j = 0; j < J; j++) P.group_verbatim[j / P.k] |= P.mode[j] == kFramed;
     P.T_threads = static_cast<int>(std::min<size_t>(static_cast<size_t>(std::max(1, bc.fetch_threads)), P.NG));
-    P.tl = TableLayout(J, P.F, n_segs, n_strided, n_casts, n_scales);
+    P.tl = TableLayout(J, P.F, scatter_bytes);
     return Err::ok();
 }
 
@@ -1081,7 +1154,7 @@ struct GpuFsReader::Call {
     }
 };
 
-Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* user_stream, const Scatter* pages) {
+Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* user_stream, const Scatter* scatter) {
     const size_t J = jobs.size();
     if (J == 0) return Err::ok();
     const double t_start = now_sec();
@@ -1103,11 +1176,9 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     CU_TRY(cudaStreamWaitEvent(G.vstream, G.entry_ev, 0));
     const B200Conf& bc = ctx_->conf.b200;
     const int poly = bc.verify_poly ? 1 : 0;
-    const size_t n_segs = pages ? pages->segs.size() : 0, n_strided = pages ? pages->strided.size() : 0, n_casts = pages ? pages->casts.size() : 0;
-    const size_t n_scales = pages ? pages->scales.size() : 0;
 
     CallPlan P;
-    CV_RETURN_IF_ERR(plan_call(jobs, n_segs, n_strided, n_casts, n_scales, &P));
+    CV_RETURN_IF_ERR(plan_call(jobs, scatter ? scatter->bytes() : 0, &P));
     Call c(*this, jobs, P, d_dst);
     if (!(bc.zero_copy && !P.call_framed)) CV_RETURN_IF_ERR(c.ensure_ring());
 
@@ -1134,23 +1205,8 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     // every whole block the manifest holds a CRC for is compared; holes, partial ranges and blocks without a manifest CRC are
     // masked out one by one (their CRCs are still computed, and summed when they lie inside [f0,f1))
     const bool compare = bc.verify && n_compared > 0;
+    if (scatter) scatter->write(tl.scatter(h));  // the scatter's tables ride in the same pinned image and the same copy
     CU_TRY(cudaMemcpyAsync(T, h, tl.o_crc, cudaMemcpyHostToDevice, G.vstream));
-    if (n_segs) {  // the scatter's segment table rides in the same pinned image
-        memcpy(tl.segs(h), pages->segs.data(), sizeof(CvSeg) * n_segs);
-        CU_TRY(cudaMemcpyAsync(tl.segs(T), tl.segs(h), sizeof(CvSeg) * n_segs, cudaMemcpyHostToDevice, G.vstream));
-    }
-    if (n_strided) {  // and so does its table of strided segments
-        memcpy(tl.strided(h), pages->strided.data(), sizeof(CvStridedSeg) * n_strided);
-        CU_TRY(cudaMemcpyAsync(tl.strided(T), tl.strided(h), sizeof(CvStridedSeg) * n_strided, cudaMemcpyHostToDevice, G.vstream));
-    }
-    if (n_casts) {  // and its table of cast segments
-        memcpy(tl.casts(h), pages->casts.data(), sizeof(CvCastSeg) * n_casts);
-        CU_TRY(cudaMemcpyAsync(tl.casts(T), tl.casts(h), sizeof(CvCastSeg) * n_casts, cudaMemcpyHostToDevice, G.vstream));
-    }
-    if (n_scales) {  // and the cast segments' scales, when K5's scaled instance runs
-        memcpy(tl.scales(h), pages->scales.data(), sizeof(CvScaleSeg) * n_scales);
-        CU_TRY(cudaMemcpyAsync(tl.scales(T), tl.scales(h), sizeof(CvScaleSeg) * n_scales, cudaMemcpyHostToDevice, G.vstream));
-    }
     CU_TRY(cudaMemsetAsync(tl.crc(T), 0, 4 * tl.res_words(), G.vstream));
     CvStreamDesc* sd = tl.streams(h);
     if (P.any_verbatim) {
@@ -1224,14 +1280,8 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     // ---- finish: compare the CRCs with the manifest, scatter, copy the results back, order the caller's stream after it all
     if (compare)
         CVK_TRY(cvk_verify_crcs_masked(d_crc + f0, tl.expect(T) + f0, tl.skip(T) + f0, static_cast<uint32_t>(f1 - f0), d_crc + J, nullptr, G.vstream));
-    if (n_segs)  // every copy group was waited for and CRC'd on vstream by now: scatter the landed bytes to their destinations
-        CVK_TRY(cvk_gather_pages(d_dst, tl.segs(T), static_cast<uint32_t>(n_segs), pages->total, pages->d_out, G.vstream));
-    if (n_strided)  // spans of several rows each
-        CVK_TRY(cvk_gather_strided(d_dst, tl.strided(T), static_cast<uint32_t>(n_strided), pages->strided_total, pages->d_out, G.vstream));
-    if (n_casts && n_scales)  // spans of converting ranges, FP8 or scaled among them: K5's scaled instance out of the verified staging
-        CVK_TRY(cvk_gather_cast_scaled(d_dst, tl.casts(T), tl.scales(T), static_cast<uint32_t>(n_casts), pages->cast_elems, pages->d_out, G.vstream));
-    else if (n_casts)  // spans of converting ranges: K5 out of the verified staging
-        CVK_TRY(cvk_gather_cast(d_dst, tl.casts(T), static_cast<uint32_t>(n_casts), pages->cast_elems, pages->d_out, G.vstream));
+    if (scatter)  // every copy group was waited for and CRC'd on vstream by now: deliver the landed bytes to their destinations
+        CV_RETURN_IF_ERR(scatter->launch(d_dst, tl.scatter(T), G.vstream));
     CU_TRY(cudaMemcpyAsync(G.h_result, d_crc, 4 * tl.res_words(), cudaMemcpyDeviceToHost, G.vstream));
     CU_TRY(cudaEventRecord(G.done_ev, G.vstream));
     CU_TRY(cudaStreamWaitEvent(static_cast<cudaStream_t>(user_stream), G.done_ev, 0));
@@ -1329,42 +1379,18 @@ Err GpuFsReader::readv_device(const ReadvRange* ranges, int32_t n_ranges, void* 
         if (b.direct) jobs.push_back(Job{&fb.block_locs[b.block], 0, spans[b.first_span].len, dst_of(spans[b.first_span]), true});
     size_t next = 0;
     do {
-        Scatter sc;
-        sc.d_out = base;
-        bool any_scaled = false;  // a cast span of this round has an FP8 source or a scale
+        Scatter sc(base);
         for (size_t slot = 0; slot < per_round && next < boundary.size(); slot++, next++) {
             const ReadvBlock& b = blocks[boundary[next]];
             const int64_t at = rel(stage + slot * static_cast<size_t>(stage_block));
             jobs.push_back(Job{&fb.block_locs[b.block], 0, fb.block_locs[b.block].block.len, at, true});
             for (size_t k = b.first_span; k < b.first_span + b.n_spans; k++) {
                 const ReadvSpan& s = spans[k];
-                const ReadvRange& r = ranges[s.range];
-                const uint64_t src = static_cast<uint64_t>(at + s.block_off), dst = static_cast<uint64_t>(dst_of(s)), len = static_cast<uint64_t>(s.len);
-                if (r.cast()) {
-                    const uint64_t elems = len / static_cast<uint64_t>(dtype_size(r.src_dtype)), rows = static_cast<uint64_t>(s.rows);
-                    sc.casts.push_back(CvCastSeg{src, dst, elems, rows, static_cast<uint64_t>(r.file_pitch), static_cast<uint64_t>(r.dst_pitch),
-                                                 sc.cast_chunks, r.src_dtype, r.dst_dtype});
-                    sc.cast_elems += elems * rows;
-                    sc.cast_chunks += rows * CV_CAST_ROW_CHUNKS(elems);
-                    // the view position of the span's first element: first_elem + (its file offset - file_off) / src size
-                    const ReadvScale& g = r.scale;
-                    const int64_t ss = dtype_size(r.src_dtype), at_file = fb.starts[b.block] + s.block_off;
-                    sc.scales.push_back(r.scaled() ? CvScaleSeg{g.ptr, uint64_t(g.block_rows), uint64_t(g.block_cols), uint64_t(g.cols),
-                                                                uint64_t(g.view_cols), uint64_t(g.first_elem + (at_file - r.file_off) / ss),
-                                                                uint64_t(r.file_pitch / ss), g.dtype, 0}
-                                                   : CvScaleSeg{});
-                    any_scaled |= r.scaled() || is_f8(r.src_dtype);
-                } else if (s.rows == 1) {
-                    sc.segs.push_back(CvSeg{src, dst, len});
-                    sc.total += len;
-                } else {
-                    sc.strided.push_back(CvStridedSeg{src, dst, len, static_cast<uint64_t>(s.rows), static_cast<uint64_t>(r.file_pitch), static_cast<uint64_t>(r.dst_pitch)});
-                    sc.strided_total += len * static_cast<uint64_t>(s.rows);
-                }
+                sc.add(static_cast<uint64_t>(at + s.block_off), static_cast<uint64_t>(dst_of(s)), static_cast<uint64_t>(s.len), static_cast<uint64_t>(s.rows),
+                       ranges[s.range], fb.starts[b.block] + s.block_off);
             }
         }
-        if (!any_scaled) sc.scales.clear();  // plain K5, exactly as without scales
-        CV_RETURN_IF_ERR(run_jobs(jobs, base, stream, sc.segs.empty() && sc.strided.empty() && sc.casts.empty() ? nullptr : &sc));
+        CV_RETURN_IF_ERR(run_jobs(jobs, base, stream, &sc));
         jobs.clear();
     } while (next < boundary.size());
     *n = total;

@@ -130,24 +130,10 @@ class GpuFsReader {
         bool full;           // whole block -> CRC comparable with the manifest
     };
     GpuFsReader() = default;
-    // scatter riding on a read: after the bytes landed in d_dst and were CRC'd, segs[i] copies d_dst + src_off to d_out + dst_off
-    // (K3), in the same launch train, no extra sync.  Page buffers of a FUSE reply (Reader::fuse_read + ResponseData::as_iovec on the
-    // device), or the spans of the boundary blocks of a vectored read: one-row spans as segs (K3), spans of several rows as strided
-    // (K3 over 2D descriptors), spans of converting ranges as casts (K5).  When a cast span has an FP8 source or a scale, `scales`
-    // holds one CvScaleSeg per cast (null scale for the others) and K5's scaled instance runs instead; otherwise `scales` is empty.
-    struct Scatter {
-        uint8_t* d_out = nullptr;
-        std::vector<CvSeg> segs;
-        uint64_t total = 0;  // sum of segs[i].len
-        std::vector<CvStridedSeg> strided;
-        uint64_t strided_total = 0;  // sum of strided[i].len * strided[i].rows
-        std::vector<CvCastSeg> casts;
-        uint64_t cast_elems = 0, cast_chunks = 0;  // sum of casts[i].elems * rows, and the next segment's `first`
-        std::vector<CvScaleSeg> scales;
-    };
+    struct Scatter;   // delivery riding on a read: spans of the landed bytes copied or converted to their destinations
     struct CallPlan;  // what one run_jobs call does, decided up front (plan_call)
     struct Call;      // one run_jobs call in flight: fetch workers and the ingest paths of a copy group
-    Err plan_call(const std::vector<Job>& jobs, size_t n_segs, size_t n_strided, size_t n_casts, size_t n_scales, CallPlan* out) const;
+    Err plan_call(const std::vector<Job>& jobs, size_t scatter_bytes, CallPlan* out) const;
     Err run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* stream, const Scatter* scatter = nullptr);
     Err read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const Scatter* scatter);
     FsContext* ctx_ = nullptr;

@@ -174,6 +174,26 @@ class Reader:
         _check(_lib.lib().cv_shard_plan(self._h, rank, world, arrs[0], arrs[1], arrs[2], arrs[3], n.value, ctypes.byref(n), ctypes.byref(tot)))
         return [tuple(a[i] for a in arrs) for i in range(n.value)]
 
+    def _device(self, fn, arr, n, stream):
+        """One call of the device read entry point `fn` over the n ranges of `arr` -> bytes delivered."""
+        got = ctypes.c_int64()
+        _check(fn(self._h, arr, n, ctypes.c_void_p(stream), ctypes.byref(got)))
+        return got.value
+
+    def _plan(self, fn, arr, n, rows):
+        """The plan entry point `fn` over the n ranges of `arr`, called once for the span count and once to fill the spans.
+        -> (spans, n_blocks, fetch_bytes) with spans as (block_index, block_off, len[, rows], range_index, direct); `rows` says whether
+        `fn` has the rows column."""
+        ns, nb, fb = ctypes.c_int32(), ctypes.c_int64(), ctypes.c_int64()
+        n64 = 4 if rows else 3
+        _check(fn(self._h, arr, n, *[None] * (n64 + 2), 0, ctypes.byref(ns), ctypes.byref(nb), ctypes.byref(fb)))
+        cap = max(1, ns.value)
+        a64 = [(ctypes.c_int64 * cap)() for _ in range(n64)]
+        a32 = [(ctypes.c_int32 * cap)() for _ in range(2)]
+        _check(fn(self._h, arr, n, *a64, *a32, cap, ctypes.byref(ns), ctypes.byref(nb), ctypes.byref(fb)))
+        spans = [tuple(a[i] for a in a64) + (a32[0][i], bool(a32[1][i])) for i in range(ns.value)]
+        return spans, nb.value, fb.value
+
     @staticmethod
     def _ranges(ranges):
         arr = (_lib.CvRange * max(1, len(ranges)))()
@@ -184,24 +204,13 @@ class Reader:
     def readv_device(self, ranges, stream: int = 0) -> int:
         """Vectored device read: `ranges` is a list of (file_off, len, d_ptr); every range lands at its d_ptr in one pipelined pass and
         every block a range touches is CRC-verified whole (see verify()).  Does not move pos.  -> sum of the lengths."""
-        n = ctypes.c_int64()
-        _check(_lib.lib().cv_readv_device(self._h, self._ranges(ranges), len(ranges), ctypes.c_void_p(stream), ctypes.byref(n)))
-        return n.value
+        return self._device(_lib.lib().cv_readv_device, self._ranges(ranges), len(ranges), stream)
 
     def readv_plan(self, ranges):
         """What readv_device(ranges) executes (host-only; the d_ptr of each range is not looked at).
         -> (spans, n_blocks, fetch_bytes): spans in file order as (block_index, block_off, len, range_index, direct); fetch_bytes = the
         summed length of the touched blocks, which is what the read moves."""
-        arr = self._ranges(ranges)
-        ns, nb, fb = ctypes.c_int32(), ctypes.c_int64(), ctypes.c_int64()
-        _check(_lib.lib().cv_readv_plan(self._h, arr, len(ranges), None, None, None, None, None, 0, ctypes.byref(ns), ctypes.byref(nb), ctypes.byref(fb)))
-        cap = max(1, ns.value)
-        a64 = [(ctypes.c_int64 * cap)() for _ in range(3)]
-        a32 = [(ctypes.c_int32 * cap)() for _ in range(2)]
-        _check(_lib.lib().cv_readv_plan(self._h, arr, len(ranges), a64[0], a64[1], a64[2], a32[0], a32[1], cap, ctypes.byref(ns), ctypes.byref(nb),
-                                        ctypes.byref(fb)))
-        spans = [(a64[0][i], a64[1][i], a64[2][i], a32[0][i], bool(a32[1][i])) for i in range(ns.value)]
-        return spans, nb.value, fb.value
+        return self._plan(_lib.lib().cv_readv_plan, self._ranges(ranges), len(ranges), rows=False)
 
     @staticmethod
     def _strided_ranges(ranges):
@@ -215,26 +224,13 @@ class Reader:
         """Strided device read: `ranges` is a list of (file_off, row_len, rows, file_pitch, d_ptr, dst_pitch); row k of a range is file
         bytes [file_off + k*file_pitch, +row_len) and lands at d_ptr + k*dst_pitch.  Verified and ordered like readv_device.
         -> sum of rows * row_len."""
-        n = ctypes.c_int64()
-        _check(_lib.lib().cv_readv_strided_device(self._h, self._strided_ranges(ranges), len(ranges), ctypes.c_void_p(stream), ctypes.byref(n)))
-        return n.value
+        return self._device(_lib.lib().cv_readv_strided_device, self._strided_ranges(ranges), len(ranges), stream)
 
     def readv_strided_plan(self, ranges):
         """What readv_strided_device(ranges) executes (host-only; d_ptr is not looked at).  -> (spans, n_blocks, fetch_bytes) with spans in
         file order as (block_index, block_off, len, rows, range_index, direct): rows k < rows of the span are bytes
         [block_off + k*file_pitch, +len) of the block."""
-        arr = self._strided_ranges(ranges)
-        ns, nb, fb = ctypes.c_int32(), ctypes.c_int64(), ctypes.c_int64()
-        L = _lib.lib()
-        _check(L.cv_readv_strided_plan(self._h, arr, len(ranges), None, None, None, None, None, None, 0, ctypes.byref(ns), ctypes.byref(nb),
-                                       ctypes.byref(fb)))
-        cap = max(1, ns.value)
-        a64 = [(ctypes.c_int64 * cap)() for _ in range(4)]
-        a32 = [(ctypes.c_int32 * cap)() for _ in range(2)]
-        _check(L.cv_readv_strided_plan(self._h, arr, len(ranges), a64[0], a64[1], a64[2], a64[3], a32[0], a32[1], cap, ctypes.byref(ns),
-                                       ctypes.byref(nb), ctypes.byref(fb)))
-        spans = [(a64[0][i], a64[1][i], a64[2][i], a64[3][i], a32[0][i], bool(a32[1][i])) for i in range(ns.value)]
-        return spans, nb.value, fb.value
+        return self._plan(_lib.lib().cv_readv_strided_plan, self._strided_ranges(ranges), len(ranges), rows=True)
 
     @staticmethod
     def _fill_cast(a, i, rng):
@@ -264,9 +260,7 @@ class Reader:
         dtypes.  A range with src_dtype == dst_dtype is a range of readv_strided_device; any other converts its elements on the GPU (float32,
         float16 and bfloat16 into one another, round-to-nearest-even; float8_e4m3fn and float8_e5m2 into those three, exactly): its file side is in source bytes, d_ptr and dst_pitch in destination
         bytes.  Every block a converting range touches is verified before it is converted.  -> bytes delivered."""
-        n = ctypes.c_int64()
-        _check(_lib.lib().cv_readv_cast_device(self._h, self._cast_ranges(ranges), len(ranges), ctypes.c_void_p(stream), ctypes.byref(n)))
-        return n.value
+        return self._device(_lib.lib().cv_readv_cast_device, self._cast_ranges(ranges), len(ranges), stream)
 
     def readv_scaled_device(self, ranges, stream: int = 0) -> int:
         """Scaled device read (FP8 checkpoints): `ranges` is a list of readv_cast_device ranges with one more item, `scale`: None (the
@@ -284,25 +278,12 @@ class Reader:
             if rng[8] is not None:
                 ptr, dt, a.scale_rows, a.scale_cols, a.block_rows, a.block_cols, a.cols, a.first_elem = rng[8]
                 a.d_scale, a.scale_dtype = ptr, scodes.get(dt, -1)
-        n = ctypes.c_int64()
-        _check(_lib.lib().cv_readv_scaled_device(self._h, arr, len(ranges), ctypes.c_void_p(stream), ctypes.byref(n)))
-        return n.value
+        return self._device(_lib.lib().cv_readv_scaled_device, arr, len(ranges), stream)
 
     def readv_cast_plan(self, ranges):
         """What readv_cast_device(ranges) executes (host-only; d_ptr is looked at for its alignment only).  -> (spans, n_blocks, fetch_bytes)
         as readv_strided_plan."""
-        arr = self._cast_ranges(ranges)
-        ns, nb, fb = ctypes.c_int32(), ctypes.c_int64(), ctypes.c_int64()
-        L = _lib.lib()
-        _check(L.cv_readv_cast_plan(self._h, arr, len(ranges), None, None, None, None, None, None, 0, ctypes.byref(ns), ctypes.byref(nb),
-                                    ctypes.byref(fb)))
-        cap = max(1, ns.value)
-        a64 = [(ctypes.c_int64 * cap)() for _ in range(4)]
-        a32 = [(ctypes.c_int32 * cap)() for _ in range(2)]
-        _check(L.cv_readv_cast_plan(self._h, arr, len(ranges), a64[0], a64[1], a64[2], a64[3], a32[0], a32[1], cap, ctypes.byref(ns),
-                                    ctypes.byref(nb), ctypes.byref(fb)))
-        spans = [(a64[0][i], a64[1][i], a64[2][i], a64[3][i], a32[0][i], bool(a32[1][i])) for i in range(ns.value)]
-        return spans, nb.value, fb.value
+        return self._plan(_lib.lib().cv_readv_cast_plan, self._cast_ranges(ranges), len(ranges), rows=True)
 
     def fuse_read_device(self, pos: int, size: int, d_scratch: int, d_page_base: int, page_offsets, page_size: int,
                          stream: int = 0) -> int:

@@ -6,6 +6,7 @@
 
 #include <atomic>
 
+#include "cuda_runtime.h"
 #include "../../include/curvine_b200_kernels.h"
 #include "../../curvine_b200/csrc/crc_gf.h"
 
@@ -167,6 +168,15 @@ int cvk_gather_pages(const uint8_t* d_src, const CvSeg* d_segs, uint32_t n, uint
     for (uint32_t i = 0; i < n; i++) memmove(d_dst + d_segs[i].dst_off, d_src + d_segs[i].src_off, d_segs[i].len);
     g_launches += 4;
     return 0;
+}
+
+// The strided gather and both instances of K5 have no stand-in here: any segment is reported as not supported, nothing is copied.
+int cvk_gather_strided(const uint8_t*, const CvStridedSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) { return n ? int(cudaErrorNotSupported) : 0; }
+
+int cvk_gather_cast(const uint8_t*, const CvCastSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) { return n ? int(cudaErrorNotSupported) : 0; }
+
+int cvk_gather_cast_scaled(const uint8_t*, const CvCastSeg*, const CvScaleSeg*, uint32_t n, uint64_t, uint8_t*, cv_stream_t) {
+    return n ? int(cudaErrorNotSupported) : 0;
 }
 
 int cvk_deinterleave_blocks(const uint8_t* g, uint64_t shard_stride, uint32_t world, uint64_t block_size, uint64_t n_blocks, uint64_t file_len,

@@ -34,7 +34,7 @@ def _run_suite_retrying_flakes(cmd, env, timeout):
     return re.sub(r"(\d+) failed, (\d+) passed", lambda m: "%d passed" % (int(m.group(1)) + int(m.group(2))), r.stdout)
 
 
-def test_gpu_reader_suite_against_the_mock_runtime():
+def test_gpu_reader_suite_against_the_mock_runtime_and_its_launcher_stand_ins():
     sys.path.insert(0, os.path.join(ROOT, "tests", "mock_cuda"))
     try:
         import build as mock_build
@@ -49,7 +49,7 @@ def test_gpu_reader_suite_against_the_mock_runtime():
     assert m and int(m.group(1)) >= 60, tail
 
 
-def test_device_reader_releases_every_device_and_pinned_allocation_and_registration():
+def test_device_reader_on_the_mock_runtime_releases_every_device_and_pinned_allocation_and_registration():
     """tests/mock_cuda/leak_check.py: mixed workload over four pipeline configurations incl. failed and abandoned reads and a device
     write; after every cv_fs_close the mock runtime must hold no device allocation, no pinned allocation and no registered range."""
     sys.path.insert(0, os.path.join(ROOT, "tests", "mock_cuda"))
