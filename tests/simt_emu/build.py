@@ -187,6 +187,12 @@ MUTATIONS = {
     # the shifted walk loses its row count above 1023 rows of 512 bytes: wrong only for segments of >= 512 KiB (s >= 19)
     "shifted_walk_drops_rows_past_1023": ("kernels.cu", "const uint32_t R = L >> 9, nv = (L & 511u) >> 4;\n    const uint32_t nvec = (L >> 4) + 1;",
                                           "const uint32_t R = (L >> 9) & 0x3ffu, nv = (L & 511u) >> 4;  /* planted */\n    const uint32_t nvec = (L >> 4) + 1;"),
+    # K5's forward segment search gives up after 6 halvings: a grid stride that skips more than 64 segments lands short of its segment
+    "cast_segment_search_spans_64_segments": ("kernels.cu", "            while (lo < hi) {\n                const uint32_t mid",
+                                              "            for (int it = 0; lo < hi && it < 6; it++) {  /* planted */\n                const uint32_t mid"),
+    # readv_device keeps a span's offset inside its range's destination in 32 bits: wrong for rows 4 GiB or more past the range's start
+    "readv_row_offset_32_bits": ("host/gpu_reader.cu", "auto dst_of = [&](const ReadvSpan& s) { return rel(ranges[s.range].dst) + s.dst_off; };",
+                                 "auto dst_of = [&](const ReadvSpan& s) { return rel(ranges[s.range].dst) + int64_t(uint32_t(s.dst_off)); /* planted */ };"),
 }
 
 

@@ -24,14 +24,14 @@ AIMED = {
 }
 
 
-def _outcomes(lib):
-    """{test id: PASSED / FAILED / ERROR / SKIPPED / CRASHED} of the launch-shape file against `lib`"""
+def _outcomes(lib, files=(FILE,)):
+    """{test id: PASSED / FAILED / ERROR / SKIPPED / CRASHED} of `files` (the launch-shape file) against `lib`"""
     env = dict(os.environ, CV_TEST_MOCK_CUDA_LIB=lib, CV_SIMT_EMU_THREADS="4")
     for k in ("MOCK_CUDA_ASYNC", "MOCK_CUDA_JITTER_US", "CV_SIMT_EMU_SMS"):
         env.pop(k, None)
     done = {}
     while True:
-        cmd = [sys.executable, "-m", "pytest", FILE, "-m", "gpu", "-v", "-p", "no:cacheprovider"]
+        cmd = [sys.executable, "-m", "pytest"] + list(files) + ["-m", "gpu", "-v", "-p", "no:cacheprovider"]
         cmd += ["--deselect=" + t for t in done]
         r = subprocess.run(cmd, cwd=ROOT, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=300)
         for t, what in re.findall(r"^(\S+::\S+) (PASSED|FAILED|ERROR|SKIPPED)\b", r.stdout, re.M):
