@@ -589,7 +589,7 @@ static inline void backoff_wait(F cond) {
 
 }  // namespace
 
-enum FetchMode { kFetchShortCircuit = 0, kFetchFramedVerbatim = 1 };
+enum JobMode : uint8_t { kPlain = 0, kFramed = 1, kHole = 3 };
 
 // n bytes of the file at `path` from file_off -> buf
 static Err pread_full(const std::string& path, int64_t file_off, uint8_t* buf, int64_t n) {
@@ -630,17 +630,17 @@ static Err open_on(FsContext* ctx, BlockClient* c, const LocatedBlock& lb, int64
 }
 
 // Fetch one job's bytes into `slot`.
-//   short-circuit    payload only (pread of the block file the worker named)
-//   framed verbatim  the response stream exactly as received: 22-byte prefixes + payloads (unpacked on the GPU by K2, which
-//                    also clips the last chunk of a range that stops short of the block end)
+//   kPlain   short-circuit: payload only (pread of the block file the worker named)
+//   kFramed  verbatim: the response stream exactly as received: 22-byte prefixes + payloads (unpacked on the GPU by K2, which
+//            also clips the last chunk of a range that stops short of the block end)
 // A replica whose block file cannot be read is given up for the next one.
-static Err fetch_job(FsContext* ctx, const LocatedBlock& lb, int64_t block_off, int64_t n, FetchMode mode, int64_t chunk, uint8_t* slot,
+static Err fetch_job(FsContext* ctx, const LocatedBlock& lb, int64_t block_off, int64_t n, JobMode mode, int64_t chunk, uint8_t* slot,
                      std::unique_ptr<BlockClient>* conn, int64_t* req_id_out, size_t* wire_bytes) {
     return for_each_replica(ctx, lb, conn, [&](BlockClient* c) -> Err {
         const int64_t req_id = new_req_id();
         *req_id_out = req_id;
         BlockReadResponse resp;
-        if (mode == kFetchShortCircuit) {
+        if (mode == kPlain) {
             CV_RETURN_IF_ERR(open_on(ctx, c, lb, block_off, req_id, &resp));
             CV_RETURN_IF_ERR(pread_full(resp.path, (resp.has_arena ? resp.arena_off : 0) + block_off, slot, n));  // arena block: an extent of the segment file
             *wire_bytes = static_cast<size_t>(n);
@@ -695,14 +695,14 @@ Err GpuFsReader::harvest() {
     GpuIngest& G = *ing_;
     cudaSetDevice(G.device);
     CU_TRY(cudaStreamSynchronize(G.vstream));
-    const uint32_t* crc = reinterpret_cast<const uint32_t*>(G.h_result);
-    const size_t J = pending_.jobs;
+    const TableLayout& tl = pending_.tl;
+    uint32_t* crc = reinterpret_cast<uint32_t*>(G.h_result);
     for (size_t j = pending_.f0; j < pending_.f1; j++) sum_crc_ += crc[j];
     n_verified_ += pending_.n_compared;
     stats_.verified += pending_.n_compared;
-    n_bad_ += crc[J];  // mismatch counter written by cvk_verify_crcs
-    const uint32_t* ferr = crc + J + 4;
-    for (size_t f = 0; f < pending_.frames; f++)
+    n_bad_ += *tl.nbad(crc);
+    const uint32_t* ferr = tl.ferr(crc);
+    for (size_t f = 0; f < tl.F; f++)
         if (ferr[f]) {
             n_bad_frames_++;
             if (!first_frame_err_) first_frame_err_ = ferr[f];
@@ -735,35 +735,16 @@ static Err check_device_dst(const void* p, int device) {
     return Err::ok();
 }
 
-enum JobMode : uint8_t { kPlain = 0, kFramed = 1, kHole = 3 };
-
-// Layout of the per-call device tables (shared by all readers of the context) and of their pinned host image:
-//   off[J] len[J] expect[J] skip[J] | scatter section | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F]
-// off .. the scatter section are uploaded in one copy before the fetch starts; crc .. ferr are the results copied back.
-struct TableLayout {
-    size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_scatter = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, bytes = 0;
-    TableLayout() = default;
-    TableLayout(size_t j, size_t f, size_t scatter_bytes) : J(j), F(f) {
-        const auto up = table_up;
-        o_len = up(8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_scatter = up(o_skip + J), o_crc = up(o_scatter + scatter_bytes);
-        o_streams = up(o_crc + 4 * res_words()), o_fdesc = up(o_streams + sizeof(CvStreamDesc) * J);
-        bytes = up(o_fdesc + sizeof(CvFrameDesc) * F);
-    }
-    size_t res_words() const { return J + 4 + F; }
-    uint64_t* off(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t); }
-    uint64_t* len(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t + o_len); }
-    uint32_t* expect(uint8_t* t) const { return reinterpret_cast<uint32_t*>(t + o_exp); }
-    uint8_t* skip(uint8_t* t) const { return t + o_skip; }
-    uint8_t* scatter(uint8_t* t) const { return t + o_scatter; }
-    uint32_t* crc(uint8_t* t) const { return reinterpret_cast<uint32_t*>(t + o_crc); }
-    uint32_t* ferr(uint8_t* t) const { return crc(t) + J + 4; }
-    CvStreamDesc* streams(uint8_t* t) const { return reinterpret_cast<CvStreamDesc*>(t + o_streams); }
-    CvFrameDesc* fdesc(uint8_t* t) const { return reinterpret_cast<CvFrameDesc*>(t + o_fdesc); }
-};
+GpuFsReader::TableLayout::TableLayout(size_t j, size_t f, size_t scatter_bytes) : J(j), F(f) {
+    const auto up = table_up;
+    o_len = up(8 * J), o_exp = up(o_len + 8 * J), o_skip = up(o_exp + 4 * J), o_scatter = up(o_skip + J), o_crc = up(o_scatter + scatter_bytes);
+    o_streams = up(o_crc + 4 * res_words()), o_fdesc = up(o_streams + sizeof(CvStreamDesc) * J);
+    bytes = up(o_fdesc + sizeof(CvFrameDesc) * F);
+}
 
 // What one run_jobs call does, decided before any CUDA call.
 struct GpuFsReader::CallPlan {
-    std::vector<uint8_t> mode;             // JobMode per job
+    std::vector<JobMode> mode;             // per job
     bool call_framed = false;              // a block without a local replica (or short_circuit off): every job runs framed
     bool any_verbatim = false;             // some job is received verbatim (framed) and unpacked by K2
     std::vector<int64_t> wire_payload;     // framed jobs: payload bytes the worker sends (>= n when the range stops short of the block end)
@@ -875,13 +856,14 @@ struct H2D {
 
 }  // namespace
 
-// One run_jobs call in flight: the fetch workers, the per-call state they share with the verifier, and the ingest paths a copy group
-// can take.  Each path returns Err::ok() when the group's copies are enqueued, kUnsupported when the group must go to the next path
-// (GDS -> registered mappings / arena -> pinned ring), or the error that fails the call.
+// One run_jobs call in flight: its tables, the fetch workers, the super-slot handoff between them and the verifier, the ingest paths a
+// copy group can take, the verifier and the finish.  Each ingest path returns Err::ok() when the group's copies are enqueued,
+// kUnsupported when the group must go to the next path (GDS -> registered mappings / arena -> pinned ring), or the error that fails the
+// call.
 struct GpuFsReader::Call {
     struct Group {
-        size_t g, ss, j0, j1;  // copy group, its super-slot, its jobs [j0, j1)
-        int t;                 // fetch worker
+        size_t g, j0, j1;  // copy group, its jobs [j0, j1)
+        int t;             // fetch worker
         cudaStream_t cs;
     };
     GpuFsReader& r;
@@ -889,11 +871,14 @@ struct GpuFsReader::Call {
     const std::vector<Job>& jobs;
     const CallPlan& P;
     uint8_t* d_dst;
+    const Scatter* scatter;
+    size_t f0 = 0, f1 = 0, n_compared = 0;  // write_tables: CRCs of jobs [f0, f1) are summed, n_compared of them compared
+    bool compare = false;                   // with the manifest, by cvk_verify_crcs_masked
     std::atomic<size_t> next_group{0};
     std::atomic<bool> abort{false};
     std::mutex err_mu, held_mu;
     Err err;
-    std::vector<std::atomic<int>> copied;
+    std::vector<std::atomic<int>> copied;        // per copy group: published
     std::vector<std::atomic<int64_t>> released;  // per super-slot: last copy group whose release event is recorded
     std::vector<int64_t> req_ids;
     std::atomic<bool> use_mapped, use_gds;
@@ -903,8 +888,8 @@ struct GpuFsReader::Call {
     std::once_flag ring_once;
     Err ring_err;
 
-    Call(GpuFsReader& reader, const std::vector<Job>& js, const CallPlan& plan, uint8_t* dst)
-        : r(reader), G(*reader.ing_), jobs(js), P(plan), d_dst(dst), copied(plan.NG), released(plan.NS), req_ids(js.size(), 0),
+    Call(GpuFsReader& reader, const std::vector<Job>& js, const CallPlan& plan, uint8_t* dst, const Scatter* sc)
+        : r(reader), G(*reader.ing_), jobs(js), P(plan), d_dst(dst), scatter(sc), copied(plan.NG), released(plan.NS), req_ids(js.size(), 0),
           fetch_sec(static_cast<size_t>(plan.T_threads), 0.0), h2d(static_cast<size_t>(plan.T_threads), 0) {
         const B200Conf& bc = r.ctx_->conf.b200;
         for (auto& c : copied) c.store(0);
@@ -925,7 +910,6 @@ struct GpuFsReader::Call {
         std::call_once(ring_once, [&] { ring_err = G.ensure(P.need_slot, P.any_verbatim); });
         return ring_err;
     }
-    uint8_t* slot_base(const Group& gr) const { return G.pinned + gr.ss * P.k * G.slot_bytes; }
 
     void worker(int t, bool own_thread) {
         if (own_thread) bind_cpus(G.cpus);  // an inline call (single copy group: small reads) must not re-pin the caller
@@ -935,8 +919,8 @@ struct GpuFsReader::Call {
         for (;;) {
             const size_t g = next_group.fetch_add(1);
             if (g >= P.NG || abort.load()) break;
-            const Group gr{g, g % P.NS, g * P.k, std::min(jobs.size(), g * P.k + P.k), t, cs};
-            if (!wait_slot(gr)) break;
+            const Group gr{g, g * P.k, std::min(jobs.size(), g * P.k + P.k), t, cs};
+            if (!acquire_slot(gr)) break;
             bool all_plain = true, all_disk = true;
             for (size_t j = gr.j0; j < gr.j1; j++) {
                 all_plain = all_plain && P.mode[j] == kPlain;
@@ -962,28 +946,55 @@ struct GpuFsReader::Call {
         }
     }
 
-    // A super-slot serves every NS-th group: wait until its previous tenant has been released, then for that tenant's copies (or,
+    // ---- The super-slot handoff.  Copy group g owns super-slot super_slot(g) of the pinned ring and of its device mirror d_stage: k
+    // slots of slot_bytes, job j's own slot at slot_off(j) in both.  A super-slot serves every NS-th group.  Every group takes part
+    // whichever path moved it (arena, mapped and GDS groups too): copy_ev belongs to the super-slot, not to a path.  Nothing but these
+    // four operations touches copy_ev, free_ev, released or copied.
+    size_t super_slot(size_t g) const { return g % P.NS; }
+    size_t slot_off(size_t j) const { return (super_slot(j / P.k) * P.k + j % P.k) * G.slot_bytes; }
+
+    // Fetch worker, before the group: wait until the super-slot's previous tenant has been released, then for that tenant's copies (or,
     // for a verbatim group, its K2) to finish with the slot.
-    bool wait_slot(const Group& gr) {
+    bool acquire_slot(const Group& gr) {
         if (gr.g < P.NS) return true;
+        const size_t ss = super_slot(gr.g);
         const int64_t want = static_cast<int64_t>(gr.g - P.NS);
-        backoff_wait([&] { return released[gr.ss].load(std::memory_order_acquire) >= want || abort.load(); });
+        backoff_wait([&] { return released[ss].load(std::memory_order_acquire) >= want || abort.load(); });
         if (abort.load()) return false;
-        cudaEventSynchronize(P.group_verbatim[gr.g - P.NS] ? G.free_ev[gr.ss] : G.copy_ev[gr.ss]);
+        cudaEventSynchronize(P.group_verbatim[gr.g - P.NS] ? G.free_ev[ss] : G.copy_ev[ss]);
         return true;
     }
 
-    // Hand the group to the verifier once its copies are enqueued.  A verbatim group's super-slot is released by the verifier after
-    // K2 has unpacked it; every other group's as soon as its copy event is recorded.
+    // Fetch worker, after the group: hand it to the verifier once its copies are enqueued.  A verbatim group's super-slot is released
+    // by the verifier after K2 has unpacked it (release_verbatim); every other group's as soon as its copy event is recorded.
     bool publish(const Group& gr, const Err& e) {
-        const cudaError_t ce = e ? cudaSuccess : cudaEventRecord(G.copy_ev[gr.ss], gr.cs);
+        const size_t ss = super_slot(gr.g);
+        const cudaError_t ce = e ? cudaSuccess : cudaEventRecord(G.copy_ev[ss], gr.cs);
         if (e || ce != cudaSuccess) {
             fail(e ? e : Err::io(str_printf("event record: %s", cudaGetErrorString(ce))));
             return false;
         }
-        if (!P.group_verbatim[gr.g]) released[gr.ss].store(static_cast<int64_t>(gr.g), std::memory_order_release);
+        if (!P.group_verbatim[gr.g]) released[ss].store(static_cast<int64_t>(gr.g), std::memory_order_release);
         copied[gr.g].store(1, std::memory_order_release);
         return true;
+    }
+
+    // Verifier, before a batch: wait until groups [v0, v1) are published, then order vstream after their copies.  false: the call failed.
+    bool await_copies(size_t v0, size_t v1) {
+        for (size_t g = v0; g < v1; g++)
+            backoff_wait([&] { return copied[g].load(std::memory_order_acquire) != 0 || abort.load(); });
+        if (abort.load()) return false;
+        for (size_t g = v0; g < v1; g++) cudaStreamWaitEvent(G.vstream, G.copy_ev[super_slot(g)], 0);
+        return true;
+    }
+
+    // Verifier, after a batch's K2: release the super-slots of its verbatim groups.
+    void release_verbatim(size_t v0, size_t v1) {
+        for (size_t g = v0; g < v1; g++)
+            if (P.group_verbatim[g]) {
+                cudaEventRecord(G.free_ev[super_slot(g)], G.vstream);
+                released[super_slot(g)].store(static_cast<int64_t>(g), std::memory_order_release);
+            }
     }
 
     // GPUDirect Storage: blocks of a disk tier go file -> HBM by cuFileRead, no host ring
@@ -1113,8 +1124,7 @@ struct GpuFsReader::Call {
         CV_RETURN_IF_ERR(fill_ring(gr, q, [&](size_t j, uint8_t* at, size_t* wire) {
             const Job& job = jobs[j];
             const double t0 = now_sec();
-            const FetchMode fm = P.mode[j] == kPlain ? kFetchShortCircuit : kFetchFramedVerbatim;
-            Err e = fetch_job(r.ctx_, *job.lb, job.block_off, job.n, fm, P.chunk, at, conn, &req_ids[j], wire);
+            Err e = fetch_job(r.ctx_, *job.lb, job.block_off, job.n, P.mode[j], P.chunk, at, conn, &req_ids[j], wire);
             fetch_sec[static_cast<size_t>(gr.t)] += now_sec() - t0;
             return e ? e.ctx(str_printf("block %lld", (long long)job.lb->block.id)) : e;
         }));
@@ -1123,7 +1133,8 @@ struct GpuFsReader::Call {
 
     // Slot layout of a ring group: when its jobs are all plain, back to back in the destination and fit into the super-slot, they
     // mirror the destination layout there and one copy moves the group; otherwise each job has a slot (and a copy) of its own.
-    // fetch(j, at, &wire) puts job j's bytes at `at`; a verbatim group's frames go to the device staging in one copy after the last.
+    // fetch(j, at, &wire) puts job j's bytes at `at`; a verbatim group's frames go to the same offsets of the device staging in one copy
+    // after the last.
     template <typename Fetch>
     Err fill_ring(const Group& gr, H2D& q, Fetch fetch) {
         const Job& first = jobs[gr.j0];
@@ -1131,7 +1142,7 @@ struct GpuFsReader::Call {
         bool mirror = static_cast<size_t>(last.dst_off + last.n - first.dst_off) <= P.k * G.slot_bytes;
         for (size_t j = gr.j0; j < gr.j1 && mirror; j++)
             mirror = P.mode[j] == kPlain && (j == gr.j0 || jobs[j].dst_off == jobs[j - 1].dst_off + jobs[j - 1].n);
-        uint8_t* hs = slot_base(gr);
+        uint8_t* hs = G.pinned + slot_off(gr.j0);
         size_t wire_extent = 0;
         for (size_t j = gr.j0; j < gr.j1 && q.ok(); j++) {
             const Job& job = jobs[j];
@@ -1139,24 +1150,137 @@ struct GpuFsReader::Call {
                 q.ce = cudaMemsetAsync(d_dst + job.dst_off, 0, static_cast<size_t>(job.n), gr.cs);  // block_reader_hole.rs:69-79
                 continue;
             }
-            const size_t at = mirror ? static_cast<size_t>(job.dst_off - first.dst_off) : (j - gr.j0) * G.slot_bytes;
+            uint8_t* at = mirror ? hs + static_cast<size_t>(job.dst_off - first.dst_off) : G.pinned + slot_off(j);
             size_t wire = 0;
-            CV_RETURN_IF_ERR(fetch(j, hs + at, &wire));
+            CV_RETURN_IF_ERR(fetch(j, at, &wire));
             if (P.mode[j] == kFramed) {
-                wire_extent = at + wire;
+                wire_extent = static_cast<size_t>(at - hs) + wire;
             } else {
-                q.add(d_dst + job.dst_off, hs + at, wire);
+                q.add(d_dst + job.dst_off, at, wire);
                 if (!mirror) q.flush();
             }
         }
-        if (wire_extent) q.add(G.d_stage + (hs - G.pinned), hs, wire_extent);
+        if (wire_extent) q.add(G.d_stage + slot_off(gr.j0), hs, wire_extent);
         return Err::ok();
+    }
+
+    // ---- The tables.  off/len/expect/skip of every job, with the [f0, f1) window of the CRCs that are summed and the count of those
+    // compared, and the scatter's tables go up in one copy; the result words are zeroed; a verbatim call's stream descriptors are
+    // written here and uploaded per batch by the verifier, once the request ids are known.  The host image is pinned, owned by the
+    // context, and rewritten only after the previous call's results were harvested (its uploads have long executed by then).
+    Err write_tables() {
+        const B200Conf& bc = r.ctx_->conf.b200;
+        const TableLayout& tl = P.tl;
+        const size_t J = jobs.size();
+        CV_RETURN_IF_ERR(G.ensure_tables(tl.bytes, 4 * tl.res_words()));
+        uint8_t* T = G.d_tables;
+        uint8_t* h = G.h_tables;
+        f0 = J, f1 = 0, n_compared = 0;
+        for (size_t j = 0; j < J; j++) {
+            const LocatedBlock& lb = *jobs[j].lb;
+            tl.off(h)[j] = static_cast<uint64_t>(jobs[j].dst_off);
+            tl.len(h)[j] = static_cast<uint64_t>(jobs[j].n);
+            tl.expect(h)[j] = bc.verify_poly ? lb.crc32c : lb.crc32;
+            tl.skip(h)[j] = !(jobs[j].full && lb.has_crc && P.mode[j] != kHole);
+            if (!tl.skip(h)[j]) {
+                f0 = std::min(f0, j), f1 = std::max(f1, j + 1);
+                n_compared++;
+            }
+        }
+        if (f0 >= f1) f0 = f1 = 0;
+        // every whole block the manifest holds a CRC for is compared; holes, partial ranges and blocks without a manifest CRC are
+        // masked out one by one (their CRCs are still computed, and summed when they lie inside [f0,f1))
+        compare = bc.verify && n_compared > 0;
+        if (scatter) scatter->write(tl.scatter(h));  // the scatter's tables ride in the same pinned image and the same copy
+        CU_TRY(cudaMemcpyAsync(T, h, tl.o_crc, cudaMemcpyHostToDevice, G.vstream));
+        CU_TRY(cudaMemsetAsync(tl.crc(T), 0, 4 * tl.res_words(), G.vstream));
+        CvStreamDesc* sd = tl.streams(h);
+        if (P.any_verbatim) {
+            for (size_t j = 0; j < J; j++) {
+                CvStreamDesc& d = sd[j];
+                memset(&d, 0, sizeof(d));
+                d.wire_off = slot_off(j), d.dst_off = tl.off(h)[j];
+                d.block_len = P.mode[j] == kFramed ? static_cast<uint64_t>(P.wire_payload[j]) : 0;
+                d.tail_clip = P.mode[j] == kFramed ? static_cast<uint32_t>(P.wire_payload[j] - jobs[j].n) : 0;
+                d.chunk_size = static_cast<uint32_t>(P.chunk), d.first_seq_id = 1, d.block = static_cast<uint32_t>(j % P.B);
+                d.first_frame = P.first_frame[j], d.code = kCodeReadBlock, d.status = 0x03;
+            }
+        }
+        return Err::ok();
+    }
+
+    // ---- The verifier: this thread walks the copy groups in order, `vgroups` at a time, and fails the call on a launch error
+    void verify_batches() {
+        const B200Conf& bc = r.ctx_->conf.b200;
+        const int poly = bc.verify_poly ? 1 : 0;
+        const TableLayout& tl = P.tl;
+        const size_t J = jobs.size();
+        uint8_t* T = G.d_tables;
+        const uint64_t* h_len = tl.len(G.h_tables);
+        CvStreamDesc* sd = tl.streams(G.h_tables);
+        uint32_t* d_crc = tl.crc(T);
+        Err verr;
+        for (size_t v0 = 0; v0 < P.NG && !verr; v0 += P.vgroups) {
+            const size_t v1 = std::min(P.NG, v0 + P.vgroups);
+            if (!await_copies(v0, v1)) break;
+            const size_t g0 = v0 * P.k, g1 = std::min(J, v1 * P.k);
+            uint64_t gbytes = 0;
+            bool gframed = false;
+            for (size_t g = v0; g < v1; g++) gframed |= P.group_verbatim[g] != 0;
+            for (size_t j = g0; j < g1; j++) gbytes += h_len[j];
+            if (!gframed && bc.verify) {  // K1 over the landed bytes
+                int rc = cvk_crc_blocks(d_dst, tl.off(T) + g0, tl.len(T) + g0, static_cast<uint32_t>(g1 - g0), poly, gbytes, d_crc + g0, G.vstream);
+                if (rc) verr = Err::io(str_printf("cvk_crc_blocks: %s", cudaGetErrorString(cudaError_t(rc))));
+            }
+            if (gframed) {
+                // patch the request ids (known only after the fetch), expand this batch's stream descriptors, run K2
+                for (size_t j = g0; j < g1; j++) sd[j].req_id = req_ids[j];
+                cudaError_t ce = cudaMemcpyAsync(tl.streams(T) + g0, &sd[g0], sizeof(CvStreamDesc) * (g1 - g0), cudaMemcpyHostToDevice, G.vstream);
+                const uint32_t fr0 = P.first_frame[g0], nfr = P.first_frame[g1] - fr0;
+                int rc = ce != cudaSuccess ? int(ce) : 0;
+                if (!rc) rc = cvk_expand_streams(tl.streams(T) + g0, static_cast<uint32_t>(g1 - g0), tl.fdesc(T), P.first_frame[J], G.vstream);
+                if (!rc && nfr)
+                    rc = cvk_unpack_frames(G.d_stage, tl.fdesc(T) + fr0, nfr, static_cast<uint32_t>(g1 - g0), d_dst, poly, gbytes,
+                                           bc.verify ? d_crc + g0 : nullptr, tl.ferr(d_crc) + fr0, G.vstream);
+                if (rc) verr = Err::io(str_printf("cvk_unpack_frames: %s", cudaGetErrorString(cudaError_t(rc))));
+                release_verbatim(v0, v1);
+            }
+        }
+        if (verr) fail(verr);
+    }
+
+    // ---- The finish: compare the CRCs with the manifest, scatter, copy the result words back, order the caller's stream after it all
+    Err finish(cudaStream_t caller) {
+        const TableLayout& tl = P.tl;
+        uint8_t* T = G.d_tables;
+        uint32_t* d_crc = tl.crc(T);
+        if (compare)
+            CVK_TRY(cvk_verify_crcs_masked(d_crc + f0, tl.expect(T) + f0, tl.skip(T) + f0, static_cast<uint32_t>(f1 - f0), tl.nbad(d_crc), nullptr, G.vstream));
+        if (scatter)  // every copy group was waited for and CRC'd on vstream by now: deliver the landed bytes to their destinations
+            CV_RETURN_IF_ERR(scatter->launch(d_dst, tl.scatter(T), G.vstream));
+        CU_TRY(cudaMemcpyAsync(G.h_result, d_crc, 4 * tl.res_words(), cudaMemcpyDeviceToHost, G.vstream));
+        CU_TRY(cudaEventRecord(G.done_ev, G.vstream));
+        CU_TRY(cudaStreamWaitEvent(caller, G.done_ev, 0));
+        return Err::ok();
+    }
+
+    void add_stats(uint64_t launches0, double t_start) {
+        GpuReadStats& st = r.stats_;
+        const uint64_t* h_len = P.tl.len(G.h_tables);
+        for (size_t j = 0; j < jobs.size(); j++) st.bytes += h_len[j];
+        st.blocks += jobs.size();
+        st.kernel_launches += cvk_launch_count() - launches0;
+        for (int t = 0; t < P.T_threads; t++) st.fetch_sec += fetch_sec[static_cast<size_t>(t)], st.h2d_bytes += h2d[static_cast<size_t>(t)];
+        st.wall_sec += now_sec() - t_start;
+        st.reg_hits = G.reg.hits.load(), st.reg_misses = G.reg.misses.load();
+        st.reg_rejected = G.reg.rejected.load(), st.reg_bytes = G.reg.bytes();
+        st.ring_alloc_sec = G.ring_alloc_sec;
+        st.gds_bytes += gds_bytes.load();
     }
 };
 
 Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* user_stream, const Scatter* scatter) {
-    const size_t J = jobs.size();
-    if (J == 0) return Err::ok();
+    if (jobs.empty()) return Err::ok();
     const double t_start = now_sec();
     GpuIngest& G = *ing_;
     struct InFlight {
@@ -1175,52 +1299,12 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     for (auto cs : G.copy_streams) CU_TRY(cudaStreamWaitEvent(cs, G.entry_ev, 0));
     CU_TRY(cudaStreamWaitEvent(G.vstream, G.entry_ev, 0));
     const B200Conf& bc = ctx_->conf.b200;
-    const int poly = bc.verify_poly ? 1 : 0;
 
     CallPlan P;
     CV_RETURN_IF_ERR(plan_call(jobs, scatter ? scatter->bytes() : 0, &P));
-    Call c(*this, jobs, P, d_dst);
+    Call c(*this, jobs, P, d_dst, scatter);
     if (!(bc.zero_copy && !P.call_framed)) CV_RETURN_IF_ERR(c.ensure_ring());
-
-    // ---- tables.  The host image is pinned, owned by the context, and rewritten only after the previous call's results were
-    // harvested (its uploads have long executed by then).
-    const TableLayout& tl = P.tl;
-    CV_RETURN_IF_ERR(G.ensure_tables(tl.bytes, 4 * tl.res_words()));
-    uint8_t* T = G.d_tables;
-    uint8_t* h = G.h_tables;
-    const uint64_t* h_len = tl.len(h);
-    size_t f0 = J, f1 = 0, n_compared = 0;
-    for (size_t j = 0; j < J; j++) {
-        const LocatedBlock& lb = *jobs[j].lb;
-        tl.off(h)[j] = static_cast<uint64_t>(jobs[j].dst_off);
-        tl.len(h)[j] = static_cast<uint64_t>(jobs[j].n);
-        tl.expect(h)[j] = poly ? lb.crc32c : lb.crc32;
-        tl.skip(h)[j] = !(jobs[j].full && lb.has_crc && P.mode[j] != kHole);
-        if (!tl.skip(h)[j]) {
-            f0 = std::min(f0, j), f1 = std::max(f1, j + 1);
-            n_compared++;
-        }
-    }
-    if (f0 >= f1) f0 = f1 = 0;
-    // every whole block the manifest holds a CRC for is compared; holes, partial ranges and blocks without a manifest CRC are
-    // masked out one by one (their CRCs are still computed, and summed when they lie inside [f0,f1))
-    const bool compare = bc.verify && n_compared > 0;
-    if (scatter) scatter->write(tl.scatter(h));  // the scatter's tables ride in the same pinned image and the same copy
-    CU_TRY(cudaMemcpyAsync(T, h, tl.o_crc, cudaMemcpyHostToDevice, G.vstream));
-    CU_TRY(cudaMemsetAsync(tl.crc(T), 0, 4 * tl.res_words(), G.vstream));
-    CvStreamDesc* sd = tl.streams(h);
-    if (P.any_verbatim) {
-        for (size_t j = 0; j < J; j++) {
-            CvStreamDesc& d = sd[j];
-            memset(&d, 0, sizeof(d));
-            const size_t ss = (j / P.k) % P.NS;
-            d.wire_off = (ss * P.k + j % P.k) * G.slot_bytes, d.dst_off = tl.off(h)[j];
-            d.block_len = P.mode[j] == kFramed ? static_cast<uint64_t>(P.wire_payload[j]) : 0;
-            d.tail_clip = P.mode[j] == kFramed ? static_cast<uint32_t>(P.wire_payload[j] - jobs[j].n) : 0;
-            d.chunk_size = static_cast<uint32_t>(P.chunk), d.first_seq_id = 1, d.block = static_cast<uint32_t>(j % P.B);
-            d.first_frame = P.first_frame[j], d.code = kCodeReadBlock, d.status = 0x03;
-        }
-    }
+    CV_RETURN_IF_ERR(c.write_tables());
 
     // ---- fetch workers.  A verbatim (framed) group's slot is only released by the verifier below, so a single fetch worker running
     // inline on this thread would wait for itself once the groups outnumber the ring's super-slots: it gets its own thread then.
@@ -1229,74 +1313,19 @@ Err GpuFsReader::run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* us
     else
         for (int t = 0; t < P.T_threads; t++) threads.emplace_back([&c, t] { c.worker(t, true); });
 
-    // ---- verifier: this thread walks the copy groups in order, `vgroups` at a time
-    Err verr;
     const uint64_t launches0 = cvk_launch_count();
-    uint32_t* d_crc = tl.crc(T);
-    const size_t NS = P.NS;
-    for (size_t v0 = 0; v0 < P.NG && !verr; v0 += P.vgroups) {
-        const size_t v1 = std::min(P.NG, v0 + P.vgroups);
-        for (size_t g = v0; g < v1; g++)
-            backoff_wait([&] { return c.copied[g].load(std::memory_order_acquire) != 0 || c.abort.load(); });
-        if (c.abort.load()) break;
-        const size_t g0 = v0 * P.k, g1 = std::min(J, v1 * P.k);
-        uint64_t gbytes = 0;
-        bool gframed = false;
-        for (size_t g = v0; g < v1; g++) {
-            cudaStreamWaitEvent(G.vstream, G.copy_ev[g % NS], 0);
-            gframed |= P.group_verbatim[g] != 0;
-        }
-        for (size_t j = g0; j < g1; j++) gbytes += h_len[j];
-        if (!gframed && bc.verify) {  // K1 over the landed bytes
-            int rc = cvk_crc_blocks(d_dst, tl.off(T) + g0, tl.len(T) + g0, static_cast<uint32_t>(g1 - g0), poly, gbytes, d_crc + g0, G.vstream);
-            if (rc) verr = Err::io(str_printf("cvk_crc_blocks: %s", cudaGetErrorString(cudaError_t(rc))));
-        }
-        if (gframed) {
-            // patch the request ids (known only after the fetch), expand this batch's stream descriptors, run K2
-            for (size_t j = g0; j < g1; j++) sd[j].req_id = c.req_ids[j];
-            cudaError_t ce = cudaMemcpyAsync(tl.streams(T) + g0, &sd[g0], sizeof(CvStreamDesc) * (g1 - g0), cudaMemcpyHostToDevice, G.vstream);
-            const uint32_t fr0 = P.first_frame[g0], nfr = P.first_frame[g1] - fr0;
-            int rc = ce != cudaSuccess ? int(ce) : 0;
-            if (!rc) rc = cvk_expand_streams(tl.streams(T) + g0, static_cast<uint32_t>(g1 - g0), tl.fdesc(T), P.first_frame[J], G.vstream);
-            if (!rc && nfr)
-                rc = cvk_unpack_frames(G.d_stage, tl.fdesc(T) + fr0, nfr, static_cast<uint32_t>(g1 - g0), d_dst, poly, gbytes,
-                                       bc.verify ? d_crc + g0 : nullptr, tl.ferr(T) + fr0, G.vstream);
-            if (rc) verr = Err::io(str_printf("cvk_unpack_frames: %s", cudaGetErrorString(cudaError_t(rc))));
-            for (size_t g = v0; g < v1; g++)
-                if (P.group_verbatim[g]) {
-                    cudaEventRecord(G.free_ev[g % NS], G.vstream);
-                    c.released[g % NS].store(static_cast<int64_t>(g), std::memory_order_release);
-                }
-        }
-    }
-    if (verr) c.fail(verr);
+    c.verify_batches();
     for (auto& th : threads) th.join();
     if (c.err) {
         cudaStreamSynchronize(G.vstream);
         for (auto s : G.copy_streams) cudaStreamSynchronize(s);
         return c.err;
     }
-
-    // ---- finish: compare the CRCs with the manifest, scatter, copy the results back, order the caller's stream after it all
-    if (compare)
-        CVK_TRY(cvk_verify_crcs_masked(d_crc + f0, tl.expect(T) + f0, tl.skip(T) + f0, static_cast<uint32_t>(f1 - f0), d_crc + J, nullptr, G.vstream));
-    if (scatter)  // every copy group was waited for and CRC'd on vstream by now: deliver the landed bytes to their destinations
-        CV_RETURN_IF_ERR(scatter->launch(d_dst, tl.scatter(T), G.vstream));
-    CU_TRY(cudaMemcpyAsync(G.h_result, d_crc, 4 * tl.res_words(), cudaMemcpyDeviceToHost, G.vstream));
-    CU_TRY(cudaEventRecord(G.done_ev, G.vstream));
-    CU_TRY(cudaStreamWaitEvent(static_cast<cudaStream_t>(user_stream), G.done_ev, 0));
-    pending_.active = true, pending_.jobs = J, pending_.frames = P.F;
-    pending_.f0 = bc.verify ? f0 : 0, pending_.f1 = bc.verify ? f1 : 0, pending_.n_compared = compare ? n_compared : 0;
+    CV_RETURN_IF_ERR(c.finish(static_cast<cudaStream_t>(user_stream)));
+    pending_.active = true, pending_.tl = P.tl;
+    pending_.f0 = bc.verify ? c.f0 : 0, pending_.f1 = bc.verify ? c.f1 : 0, pending_.n_compared = c.compare ? c.n_compared : 0;
     G.pending_owner = this;
-    for (size_t j = 0; j < J; j++) stats_.bytes += h_len[j];
-    stats_.blocks += J;
-    stats_.kernel_launches += cvk_launch_count() - launches0;
-    for (int t = 0; t < P.T_threads; t++) stats_.fetch_sec += c.fetch_sec[static_cast<size_t>(t)], stats_.h2d_bytes += c.h2d[static_cast<size_t>(t)];
-    stats_.wall_sec += now_sec() - t_start;
-    stats_.reg_hits = G.reg.hits.load(), stats_.reg_misses = G.reg.misses.load();
-    stats_.reg_rejected = G.reg.rejected.load(), stats_.reg_bytes = G.reg.bytes();
-    stats_.ring_alloc_sec = G.ring_alloc_sec;
-    stats_.gds_bytes += c.gds_bytes.load();
+    c.add_stats(launches0, t_start);
     return Err::ok();
 }
 

@@ -129,10 +129,30 @@ class GpuFsReader {
         int64_t dst_off;     // where they go in d_dst
         bool full;           // whole block -> CRC comparable with the manifest
     };
+    // Layout of the per-call device tables (shared by all readers of the context) and of their pinned host image:
+    //   off[J] len[J] expect[J] skip[J] | scatter section | crc[J] nbad[4] ferr[F] | streams[J] fdesc[F]
+    // off .. the scatter section are uploaded in one copy before the fetch starts; crc .. ferr are the result words copied back.
+    struct TableLayout {
+        size_t J = 0, F = 0, o_len = 0, o_exp = 0, o_skip = 0, o_scatter = 0, o_crc = 0, o_streams = 0, o_fdesc = 0, bytes = 0;
+        TableLayout() = default;
+        TableLayout(size_t j, size_t f, size_t scatter_bytes);
+        size_t res_words() const { return J + 4 + F; }
+        uint64_t* off(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t); }
+        uint64_t* len(uint8_t* t) const { return reinterpret_cast<uint64_t*>(t + o_len); }
+        uint32_t* expect(uint8_t* t) const { return reinterpret_cast<uint32_t*>(t + o_exp); }
+        uint8_t* skip(uint8_t* t) const { return t + o_skip; }
+        uint8_t* scatter(uint8_t* t) const { return t + o_scatter; }
+        uint32_t* crc(uint8_t* t) const { return reinterpret_cast<uint32_t*>(t + o_crc); }
+        // within the result words `res` (crc(t) in the tables, or the pinned mirror they are copied back to)
+        uint32_t* nbad(uint32_t* res) const { return res + J; }      // mismatch counter (cvk_verify_crcs_masked)
+        uint32_t* ferr(uint32_t* res) const { return res + J + 4; }  // frame flags (cvk_unpack_frames)
+        CvStreamDesc* streams(uint8_t* t) const { return reinterpret_cast<CvStreamDesc*>(t + o_streams); }
+        CvFrameDesc* fdesc(uint8_t* t) const { return reinterpret_cast<CvFrameDesc*>(t + o_fdesc); }
+    };
     GpuFsReader() = default;
     struct Scatter;   // delivery riding on a read: spans of the landed bytes copied or converted to their destinations
     struct CallPlan;  // what one run_jobs call does, decided up front (plan_call)
-    struct Call;      // one run_jobs call in flight: fetch workers and the ingest paths of a copy group
+    struct Call;      // one run_jobs call in flight: its tables, fetch workers, super-slot handoff, verifier and finish
     Err plan_call(const std::vector<Job>& jobs, size_t scatter_bytes, CallPlan* out) const;
     Err run_jobs(const std::vector<Job>& jobs, uint8_t* d_dst, void* stream, const Scatter* scatter = nullptr);
     Err read_device_impl(void* d_dst, int64_t cap, void* stream, int64_t* n, const Scatter* scatter);
@@ -149,7 +169,8 @@ class GpuFsReader {
     std::vector<std::shared_ptr<const FileBlocks>> held_files_;  // read_many: keeps the LocatedBlocks alive
     struct Pending {
         bool active = false;
-        size_t jobs = 0, frames = 0, f0 = 0, f1 = 0, n_compared = 0;
+        TableLayout tl;  // of the call whose result words sit in h_result
+        size_t f0 = 0, f1 = 0, n_compared = 0;
     } pending_;
     Err harvest();
     friend class GpuIngest;

@@ -178,9 +178,9 @@ MUTATIONS = {
     # name -> (file under csrc/, old text, new text)
     "copies_do_not_wait_for_the_callers_stream": ("host/gpu_reader.cu", "for (auto cs : G.copy_streams) CU_TRY(cudaStreamWaitEvent(cs, G.entry_ev, 0));",
                                                    "/* planted: the copy streams start without waiting for what the caller enqueued before the read */;"),
-    "callers_stream_does_not_wait_for_the_read": ("host/gpu_reader.cu", "CU_TRY(cudaStreamWaitEvent(static_cast<cudaStream_t>(user_stream), G.done_ev, 0));",
+    "callers_stream_does_not_wait_for_the_read": ("host/gpu_reader.cu", "CU_TRY(cudaStreamWaitEvent(caller, G.done_ev, 0));",
                                                    "/* planted: the caller's stream continues without waiting for the read */;"),
-    "verifier_does_not_wait_for_the_copy": ("host/gpu_reader.cu", "cudaStreamWaitEvent(G.vstream, G.copy_ev[g % NS], 0);", "/* planted: the verify stream no longer waits for the group's copies */;"),
+    "verifier_does_not_wait_for_the_copy": ("host/gpu_reader.cu", "cudaStreamWaitEvent(G.vstream, G.copy_ev[super_slot(g)], 0);", "/* planted: the verify stream no longer waits for the group's copies */;"),
     # K5's scale walk divides view positions in 32 bits even when a position or the view's width is >= 2^32
     "scale_walk_divides_in_32_bits": ("kernels.cu", "{ return (a | b) >> 32 ? a / b : uint64_t(uint32_t(a) / uint32_t(b)); }",
                                       "{ return uint64_t(uint32_t(a) / uint32_t(b)); /* planted: always 32-bit */ }"),
