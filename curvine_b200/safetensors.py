@@ -19,13 +19,19 @@ class SafetensorsError(ValueError):
     """The file is not a well-formed safetensors file."""
 
 
+# every dtype of the format -> its width in bits.  F4 and F6_* pack their elements into bytes, so a tensor of theirs must end on a
+# byte boundary (numel * bits a multiple of 8), as the format's own reader requires
+BITS = {"F4": 4, "F6_E2M3": 6, "F6_E3M2": 6, "BOOL": 8, "U8": 8, "I8": 8, "F8_E4M3": 8, "F8_E5M2": 8, "F8_E8M0": 8, "I16": 16, "U16": 16,
+        "F16": 16, "BF16": 16, "I32": 32, "U32": 32, "F32": 32, "I64": 64, "U64": 64, "F64": 64, "C64": 64}
+
+
 def dtypes() -> dict:
     """safetensors dtype name -> torch dtype, for every dtype of the format this torch build has."""
     import torch
     m = {"F64": torch.float64, "F32": torch.float32, "F16": torch.float16, "BF16": torch.bfloat16, "I64": torch.int64, "I32": torch.int32,
          "I16": torch.int16, "I8": torch.int8, "U8": torch.uint8, "BOOL": torch.bool, "F8_E4M3": torch.float8_e4m3fn,
          "F8_E5M2": torch.float8_e5m2}
-    for name, attr in (("U16", "uint16"), ("U32", "uint32"), ("U64", "uint64")):
+    for name, attr in (("U16", "uint16"), ("U32", "uint32"), ("U64", "uint64"), ("F8_E8M0", "float8_e8m0fnu"), ("C64", "complex64")):
         if hasattr(torch, attr):
             m[name] = getattr(torch, attr)
     return m
@@ -37,7 +43,10 @@ def _is_int(x) -> bool:
 
 def parse_header(read: Callable[[int, int], bytes], file_len: int) -> Tuple[int, Dict[str, tuple]]:
     """Reads and validates the header of a safetensors file of `file_len` bytes; `read(off, n)` returns n bytes of the file at off.
-    -> (data_start, {name: (torch dtype, shape, begin, end)}) with begin/end relative to data_start.  Raises SafetensorsError."""
+    -> (data_start, {name: (torch dtype, shape, begin, end)}) with begin/end relative to data_start; a tensor of a dtype of the format
+    that torch cannot hold (F4, F6_E2M3, F6_E3M2) has the format's name in place of the torch dtype.  Every dtype of the format
+    parses; a tensor's shape must need exactly its bytes, numel * bits = 8 * (end - begin).  Unlike the format's own reader, this one
+    allows gaps between tensors and after the last one.  Raises SafetensorsError."""
     if file_len < 8:
         raise SafetensorsError("file of %d bytes is too short for the 8-byte header length" % file_len)
     (n,) = struct.unpack("<Q", read(0, 8))
@@ -60,7 +69,7 @@ def parse_header(read: Callable[[int, int], bytes], file_len: int) -> Tuple[int,
         if not isinstance(ent, dict):
             raise SafetensorsError("%s: entry is not an object" % name)
         dt, shape, offs = ent.get("dtype"), ent.get("shape"), ent.get("data_offsets")
-        if dt not in table:
+        if not isinstance(dt, str) or dt not in BITS:
             raise SafetensorsError("%s: unknown dtype %r" % (name, dt))
         if not isinstance(shape, list) or not all(_is_int(d) and d >= 0 for d in shape):
             raise SafetensorsError("%s: shape %r is not a list of non-negative integers" % (name, shape))
@@ -72,9 +81,12 @@ def parse_header(read: Callable[[int, int], bytes], file_len: int) -> Tuple[int,
         count = 1
         for d in shape:
             count *= d
-        if count * table[dt].itemsize != end - begin:
-            raise SafetensorsError("%s: shape %r of %s needs %d bytes, data_offsets hold %d" % (name, shape, dt, count * table[dt].itemsize, end - begin))
-        out[name] = (table[dt], tuple(shape), begin, end)
+        need = count * BITS[dt]
+        if need % 8:
+            raise SafetensorsError("%s: shape %r of %s is %d bits, which does not end on a byte boundary" % (name, shape, dt, need))
+        if need != 8 * (end - begin):
+            raise SafetensorsError("%s: shape %r of %s needs %d bytes, data_offsets hold %d" % (name, shape, dt, need // 8, end - begin))
+        out[name] = (table.get(dt, dt), tuple(shape), begin, end)
     spans = sorted((b, e, name) for name, (_, _, b, e) in out.items() if e > b)
     for (_, e0, n0), (b1, _, n1) in zip(spans, spans[1:]):
         if b1 < e0:
@@ -103,7 +115,8 @@ def _open_header(fs, path):
 
 def read_header(fs: "_fs.CurvineFileSystem", path: str) -> Dict[str, tuple]:
     """{name: (torch dtype, shape)} of safetensors file `path`, from its header alone: what a tensor-parallel rank needs to compute the
-    `slices` it passes to load_file."""
+    `slices` it passes to load_file.  A tensor whose dtype torch cannot hold (F4, F6_E2M3, F6_E3M2) is listed with the format's dtype
+    name in place of the torch dtype; load_file refuses to load it."""
     r, _, entries = _open_header(fs, path)
     r.complete()
     return {name: (dt, shape) for name, (dt, shape, _, _) in entries.items()}
@@ -197,9 +210,12 @@ def plan_ranges(data_start: int, entries: Dict[str, tuple], selected, slices=Non
     result bytes.  With `scales` ({float8 weight: name of its scale tensor}, dtype required; scale_block = (br, bc) for block scales)
     every range gets one more item, the `scale` of Reader.readv_scaled_device with the scale tensor's NAME in place of its pointer: None,
     or (scale name, scale_rows, scale_cols, block_rows, block_cols, cols, first_elem), first_elem being a sliced weight's offset in the
-    full tensor in elements.  Raises KeyError for a sliced name the file does not hold, ValueError for a malformed slice, a sliced name
-    outside `selected`, a tensor load_file(dtype=...) cannot convert (see _cast_targets) or a weight and scale load_file(scales=...)
-    cannot dequantize (see _scale_geometry)."""
+    full tensor in elements.  Raises KeyError for a sliced name the file does not hold, ValueError for a selected tensor whose dtype
+    torch cannot hold (see parse_header), a malformed slice, a sliced name outside `selected`, a tensor load_file(dtype=...) cannot
+    convert (see _cast_targets) or a weight and scale load_file(scales=...) cannot dequantize (see _scale_geometry)."""
+    for name in selected:
+        if isinstance(entries[name][0], str):
+            raise ValueError("%s: its dtype %s has no torch dtype, so it cannot be loaded" % (name, entries[name][0]))
     slices = dict(slices or {})
     sel = set(selected)
     if scale_block is not None and scales is None:
@@ -258,15 +274,18 @@ def load_file(fs: "_fs.CurvineFileSystem", path: str, device=None, names: Option
     CRC-verified whole, including the bytes of unselected neighbours that share it.  `slices` maps a name to (dim, start, stop): that
     tensor comes back contiguous with shape[dim] = stop - start -- a tensor-parallel rank's shard, without the rest of the tensor ever
     reaching HBM (see plan_ranges).  `dtype` (torch.float32, torch.float16 or torch.bfloat16) converts every float32, float16 and bfloat16
-    tensor to it on the GPU in the same read, bit-identical to Tensor.to() on the CPU; integer and bool tensors come back as stored.  The
+    tensor to it on the GPU in the same read, bit-identical to Tensor.to() on the CPU; integer, bool and complex64 tensors come back as
+    stored, and a selected float tensor of another width (float64, float8 including F8_E8M0) is refused.  The
     stored copy never exists in HBM: a converted tensor's blocks pass through the reader's bounded staging.  `scales` maps float8 weights
     (F8_E4M3, F8_E5M2) to the names of their scale tensors in the same file (F32, F16 or BF16: one element, one per row of a 2-D weight,
     or with scale_block = (br, bc) one per br x bc tile): those weights come back in `dtype`, dequantized on the GPU as they load, each
     element (x.float() * scale.float()).to(dtype) bit for bit; they compose with `slices`.  The scales are read first, as stored, into
     temporaries; the second read then dequantizes (two calls on the caller's stream, one verification).  Float8 tensors not named in
-    `scales` are refused, as without it.  Raises IOError when a block fails verification and `verify` is set, SafetensorsError for a
-    malformed header, KeyError for a name the file does not hold, ValueError for a malformed slice, a tensor `dtype` cannot convert or a
-    weight and scale that cannot be dequantized (all before anything is allocated or read)."""
+    `scales` are refused, as without it.  Without `dtype` every tensor comes back as stored, F8_E8M0 as float8_e8m0fnu and C64 as
+    complex64.  Raises IOError when a block fails verification and `verify` is set, SafetensorsError for a malformed header, KeyError for
+    a name the file does not hold, ValueError for a selected tensor whose dtype torch cannot hold (F4, F6_E2M3, F6_E3M2; names=None
+    selects them too), a malformed slice, a tensor `dtype` cannot convert or a weight and scale that cannot be dequantized (all before
+    anything is allocated or read)."""
     import torch
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     r, data_start, entries = _open_header(fs, path)
