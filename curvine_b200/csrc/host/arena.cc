@@ -2,7 +2,6 @@
 
 #include <errno.h>
 #include <fcntl.h>
-#include <sched.h>
 #include <stdlib.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
@@ -10,6 +9,8 @@
 
 #include <atomic>
 #include <thread>
+
+#include "numa.h"
 
 namespace cv {
 
@@ -89,12 +90,7 @@ Err MemArena::add_segments(size_t n) {
     std::vector<std::thread> ts;
     for (size_t t = 0; t < T; t++)
         ts.emplace_back([&] {
-            if (!cpus_.empty()) {
-                cpu_set_t set;
-                CPU_ZERO(&set);
-                for (int c : cpus_) CPU_SET(c, &set);
-                sched_setaffinity(0, sizeof(set), &set);
-            }
+            bind_cpus(cpus_);
             for (;;) {
                 const size_t i = next.fetch_add(1);
                 if (i >= work.size()) break;

@@ -8,6 +8,7 @@
 #include <unistd.h>
 
 #include "conf.h"
+#include "numa.h"
 
 namespace cv {
 
@@ -79,28 +80,6 @@ static Err mkdirs(const std::string& path) {
         if (i < path.size()) cur.push_back(path[i]);
     }
     return Err::ok();
-}
-
-static std::vector<int> node_cpus(int node) {
-    std::vector<int> cpus;
-    if (node < 0) return cpus;
-    FILE* f = fopen(str_printf("/sys/devices/system/node/node%d/cpulist", node).c_str(), "r");
-    if (!f) return cpus;
-    char line[4096] = {0};
-    if (fgets(line, sizeof(line), f)) {
-        for (char* p = line; *p;) {
-            char* e = nullptr;
-            const long a = strtol(p, &e, 10);
-            if (e == p) break;
-            long b = a;
-            if (*e == '-') b = strtol(e + 1, &e, 10);
-            for (long x = a; x <= b; x++) cpus.push_back(static_cast<int>(x));
-            p = *e == ',' ? e + 1 : e;
-            if (*e != ',') break;
-        }
-    }
-    fclose(f);
-    return cpus;
 }
 
 Err BlockStore::init(const std::vector<std::string>& data_dirs, const std::string& cluster_id, const ArenaOpts& arena) {

@@ -4,7 +4,6 @@
 #include <nmmintrin.h>
 #include <errno.h>
 #include <fcntl.h>
-#include <sched.h>
 #include <stdlib.h>
 #include <unistd.h>
 
@@ -16,6 +15,7 @@
 #include "client.h"
 #include "gds.h"
 #include "gpu_reader.h"
+#include "numa.h"
 #include "worker.h"
 #include "writer.h"
 
@@ -764,49 +764,12 @@ static std::vector<std::vector<int>> gpu_node_cpus() {
         cudaGetLastError();
         return out;
     }
-    for (int d = 0; d < n; d++) {
-        std::vector<int> cpus;
-        char bus[64] = {0};
-        int node = -1;
-        if (cudaDeviceGetPCIBusId(bus, sizeof(bus), d) == cudaSuccess) {
-            for (char* p = bus; *p; p++) *p = static_cast<char>(tolower(*p));
-            std::ifstream f(std::string("/sys/bus/pci/devices/") + bus + "/numa_node");
-            if (f) f >> node;
-        }
-        if (node >= 0) {
-            std::ifstream f("/sys/devices/system/node/node" + std::to_string(node) + "/cpulist");
-            std::string line;
-            if (f && std::getline(f, line)) {
-                size_t p = 0;
-                while (p < line.size()) {
-                    const size_t c2 = line.find(',', p);
-                    const std::string r = line.substr(p, c2 == std::string::npos ? std::string::npos : c2 - p);
-                    const size_t dd = r.find('-');
-                    const int a = atoi(r.c_str()), b = dd == std::string::npos ? a : atoi(r.c_str() + dd + 1);
-                    for (int x = a; x <= b; x++) cpus.push_back(x);
-                    if (c2 == std::string::npos) break;
-                    p = c2 + 1;
-                }
-            }
-        }
-        out.push_back(cpus);
-    }
+    for (int d = 0; d < n; d++) out.push_back(node_cpus(gpu_numa_node(d)));
     return out;
 }
 
 // NUMA node of the PCIe root the device hangs off (-1 unknown): where its mem arena and fetch threads should live
-int64_t cv_gpu_numa_node(int32_t device) {
-    char bus[64] = {0};
-    int node = -1;
-    if (cudaDeviceGetPCIBusId(bus, sizeof(bus), device) != cudaSuccess) {
-        cudaGetLastError();
-        return -1;
-    }
-    for (char* p = bus; *p; p++) *p = static_cast<char>(tolower(*p));
-    std::ifstream f(std::string("/sys/bus/pci/devices/") + bus + "/numa_node");
-    if (f) f >> node;
-    return node;
-}
+int64_t cv_gpu_numa_node(int32_t device) { return gpu_numa_node(device); }
 
 static int g_synth_shard_world = 0;
 
@@ -881,15 +844,7 @@ int64_t cv_synth_create_file(cv_worker* w, const char* path, int64_t inode_id, i
             LocatedBlock& lb = fb.block_locs[static_cast<size_t>(b)];
             BlockWriteTarget& t = targets[static_cast<size_t>(b)];
             const int64_t blen = lb.block.len;
-            if (!node_cpus.empty()) {
-                const std::vector<int>& cpus = node_cpus[static_cast<size_t>(b % g_synth_shard_world) % node_cpus.size()];
-                if (!cpus.empty()) {
-                    cpu_set_t set;
-                    CPU_ZERO(&set);
-                    for (int c : cpus) CPU_SET(c, &set);
-                    sched_setaffinity(0, sizeof(set), &set);
-                }
-            }
+            if (!node_cpus.empty()) bind_cpus(node_cpus[static_cast<size_t>(b % g_synth_shard_world) % node_cpus.size()]);
             uint8_t* out = t.arena ? t.mem() : buf.data();
             if (mode == 1)
                 for (int64_t o = 0; o < blen; o += static_cast<int64_t>(az.size()))

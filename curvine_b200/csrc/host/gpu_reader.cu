@@ -8,12 +8,12 @@
 
 #include <algorithm>
 #include <array>
-#include <fstream>
 
 #include "../../../include/curvine_b200_kernels.h"
 #include "block_store.h"
 #include "gds.h"
 #include "net.h"
+#include "numa.h"
 #include "reg_cache.h"
 
 namespace cv {
@@ -116,30 +116,8 @@ class GpuIngest {
         register_inline = c.register_threads <= 0 || reg.capacity == 0;
         // CPUs of the GPU's NUMA node: pinned pages and fetch threads stay next to the PCIe root
         int node = c.numa_node;  // -1: the GPU's node (auto); -2: do not bind the fetch threads
-        if (node == -1) {
-            char bus[64] = {0};
-            if (cudaDeviceGetPCIBusId(bus, sizeof(bus), device) == cudaSuccess) {
-                for (char* p = bus; *p; p++) *p = static_cast<char>(tolower(*p));
-                std::ifstream f(std::string("/sys/bus/pci/devices/") + bus + "/numa_node");
-                if (f) f >> node;
-            }
-        }
-        if (node >= 0) {
-            std::ifstream f("/sys/devices/system/node/node" + std::to_string(node) + "/cpulist");
-            std::string s;
-            if (f && std::getline(f, s)) {
-                size_t p = 0;
-                while (p < s.size()) {
-                    const size_t c2 = s.find(',', p);
-                    const std::string r = s.substr(p, c2 == std::string::npos ? std::string::npos : c2 - p);
-                    const size_t d = r.find('-');
-                    const int a = atoi(r.c_str()), b = d == std::string::npos ? a : atoi(r.c_str() + d + 1);
-                    for (int x = a; x <= b; x++) cpus.push_back(x);
-                    if (c2 == std::string::npos) break;
-                    p = c2 + 1;
-                }
-            }
-        }
+        if (node == -1) node = gpu_numa_node(device);
+        cpus = node_cpus(node);
         if (c.zero_copy && !register_inline) registrar.start(c.register_threads, device, &reg, cpus, c.register_when_idle ? &reads_in_flight : nullptr);
         if (c.zero_copy && c.arena) arena.start(std::max(1, c.register_threads), device, cpus, static_cast<size_t>(std::max<int64_t>(c.arena_register_slice, 0)));
         else arena.unsupported.store(true);

@@ -4,7 +4,6 @@
 #include <cuda_runtime.h>
 #include <errno.h>
 #include <fcntl.h>
-#include <sched.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -21,19 +20,11 @@
 #include <vector>
 
 #include "common.h"
+#include "numa.h"
 
 namespace cv {
 
 inline size_t page_up(size_t bytes) { return (bytes + 4095) & ~size_t(4095); }
-
-// Pin the calling thread to `cpus` (no-op when empty): the CPUs of the GPU's NUMA node.
-inline void bind_cpus(const std::vector<int>& cpus) {
-    if (cpus.empty()) return;
-    cpu_set_t set;
-    CPU_ZERO(&set);
-    for (int c : cpus) CPU_SET(c, &set);
-    sched_setaffinity(0, sizeof(set), &set);
-}
 
 // ------------------------------------------------------------------ registered mem-tier mappings (zero-copy ingest)
 //
