@@ -67,6 +67,8 @@ class CvScaledRange(ctypes.Structure):
 
 # include/curvine_b200_kernels.h: element types of cast reads and cvk_gather_cast (the two FP8 codes: sources only)
 DTYPE_NONE, DTYPE_F32, DTYPE_F16, DTYPE_BF16, DTYPE_F8_E4M3, DTYPE_F8_E5M2 = 0, 1, 2, 3, 4, 5
+FLOAT_CODES = (DTYPE_F32, DTYPE_F16, DTYPE_BF16)  # conversion targets and scale dtypes
+F8_CODES = (DTYPE_F8_E4M3, DTYPE_F8_E5M2)  # sources only
 
 
 def cast_row_chunks(elems: int) -> int:

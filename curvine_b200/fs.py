@@ -8,6 +8,7 @@ plus the CUDA counterpart (read_device / read_device_sharded / verify) on the sa
 Errors raise FsError carrying the reference's ErrorKind (fs_error.rs:35-66).
 """
 import ctypes
+import functools
 from typing import List, Optional
 
 from . import _lib
@@ -23,6 +24,14 @@ class FsError(Exception):
 def _check(rc: int):
     if rc != 0:
         raise FsError(-rc, _lib.lib().cv_last_error().decode(errors="replace"))
+
+
+@functools.lru_cache(maxsize=None)
+def cast_dtype_codes() -> dict:
+    """{torch dtype: _lib.DTYPE_* code} of every element type cast reads know; the codes' roles are _lib.FLOAT_CODES and _lib.F8_CODES."""
+    import torch
+    return {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.bfloat16: _lib.DTYPE_BF16,
+            torch.float8_e4m3fn: _lib.DTYPE_F8_E4M3, torch.float8_e5m2: _lib.DTYPE_F8_E5M2}
 
 
 def gds_info() -> dict:
@@ -234,15 +243,10 @@ class Reader:
 
     @staticmethod
     def _fill_cast(a, i, rng):
-        import torch
         off, row_len, rows, file_pitch, ptr, dst_pitch, src, dst = rng
-        floats = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.bfloat16: _lib.DTYPE_BF16}
-        f8 = {torch.float8_e4m3fn: _lib.DTYPE_F8_E4M3, torch.float8_e5m2: _lib.DTYPE_F8_E5M2}
-        if src == dst:
-            sc = dc = floats.get(src, f8.get(src, _lib.DTYPE_NONE))
-        elif (src in floats or src in f8) and dst in floats:
-            sc, dc = floats.get(src, f8.get(src)), floats[dst]
-        else:
+        codes = cast_dtype_codes()
+        sc, dc = codes.get(src, _lib.DTYPE_NONE), codes.get(dst, _lib.DTYPE_NONE)
+        if src != dst and (sc == _lib.DTYPE_NONE or dc not in _lib.FLOAT_CODES):
             raise ValueError("range %d: conversions are from float32, float16, bfloat16, float8_e4m3fn or float8_e5m2 to float32, float16 or "
                              "bfloat16 only, not %s -> %s" % (i, src, dst))
         a.file_off, a.row_len, a.rows, a.file_pitch, a.d_dst, a.dst_pitch = off, row_len, rows, file_pitch, ptr, dst_pitch
@@ -269,15 +273,14 @@ class Reader:
         row-major view of `cols` columns.  View element (i, j) is multiplied by scale[i // block_rows, j // block_cols] in float32 and
         rounded once to the range's result dtype; element e of range row k is view element first_elem + k * file_pitch + e.  -> bytes
         delivered."""
-        import torch
-        scodes = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.bfloat16: _lib.DTYPE_BF16}
         arr = (_lib.CvScaledRange * max(1, len(ranges)))()
         for i, rng in enumerate(ranges):
             a = arr[i]
             self._fill_cast(a.cast, i, rng[:8])
             if rng[8] is not None:
                 ptr, dt, a.scale_rows, a.scale_cols, a.block_rows, a.block_cols, a.cols, a.first_elem = rng[8]
-                a.d_scale, a.scale_dtype = ptr, scodes.get(dt, -1)
+                code = cast_dtype_codes().get(dt)
+                a.d_scale, a.scale_dtype = ptr, code if code in _lib.FLOAT_CODES else -1
         return self._device(_lib.lib().cv_readv_scaled_device, arr, len(ranges), stream)
 
     def readv_cast_plan(self, ranges):

@@ -9,6 +9,7 @@ import numbers
 import struct
 from typing import Callable, Dict, Iterable, List, Optional, Tuple
 
+from . import _lib
 from . import fs as _fs
 
 # the safetensors reference reader refuses headers larger than this; a larger length is a corrupt or hostile file
@@ -126,13 +127,17 @@ def _is_integral(x) -> bool:
     return isinstance(x, numbers.Integral) and not isinstance(x, bool)
 
 
+def _dtypes_of(codes) -> tuple:
+    """the torch dtypes whose cast-read code (fs.cast_dtype_codes) is one of `codes`"""
+    return tuple(t for t, c in _fs.cast_dtype_codes().items() if c in codes)
+
+
 def _cast_targets(data_start: int, entries: Dict[str, tuple], selected, dtype, scaled=()) -> Dict[str, object]:
     """{name: dtype of the result} for load_file(dtype=...): the float32, float16 and bfloat16 tensors become `dtype`, the others stay as
     stored.  Raises ValueError for a target dtype other than those three, for a selected float tensor of another width (float64, float8:
     not converted) and for a converting tensor whose data offset is not a multiple of its element size.  The float8 weights named in
     `scaled` (load_file(scales=...)) become `dtype` too."""
-    import torch
-    floats = (torch.float32, torch.float16, torch.bfloat16)
+    floats = _dtypes_of(_lib.FLOAT_CODES)
     if dtype not in floats:
         raise ValueError("dtype %s: loads convert to float32, float16 or bfloat16 only" % (dtype,))
     out = {}
@@ -154,14 +159,12 @@ def _scale_geometry(entries: Dict[str, tuple], selected, scales, scale_block, dt
     The weight is seen as the row-major 2-D view [V_rows, cols = shape[-1]]; its scale is one element (per tensor, any shape), (V_rows, 1)
     for a 2-D weight (per row), or, with scale_block = (br, bc), (ceil(R / br), ceil(C / bc)) for a 2-D weight (blocks).  Raises
     ValueError, naming the weight and its scale, for anything else (see load_file)."""
-    import torch
     if dtype is None:
         raise ValueError("scales are given without dtype: dequantized weights need a result dtype")
     if scale_block is not None and (not isinstance(scale_block, (tuple, list)) or len(scale_block) != 2
                                     or not all(_is_integral(x) and x >= 1 for x in scale_block)):
         raise ValueError("scale_block %r is not (block_rows, block_cols) of positive integers" % (scale_block,))
-    f8 = (torch.float8_e4m3fn, torch.float8_e5m2)
-    floats = (torch.float32, torch.float16, torch.bfloat16)
+    f8, floats = _dtypes_of(_lib.F8_CODES), _dtypes_of(_lib.FLOAT_CODES)
     sel = set(selected)
     out = {}
     for w, sname in dict(scales).items():

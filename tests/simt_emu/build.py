@@ -194,7 +194,7 @@ MUTATIONS = {
     "readv_row_offset_32_bits": ("host/gpu_reader.cu", "auto dst_of = [&](const ReadvSpan& s) { return rel(ranges[s.range].dst) + s.dst_off; };",
                                  "auto dst_of = [&](const ReadvSpan& s) { return rel(ranges[s.range].dst) + int64_t(uint32_t(s.dst_off)); /* planted */ };"),
     # the cast planner places the rest of an F16 -> F32 row that crosses a block edge at its source byte offset, not its destination one
-    "cast_row_rest_offset_in_source_bytes": ("host/gpu_reader.cu", "emit(q, take, 1, row * r.dst_pitch + col / ss * ds);",
+    "cast_row_rest_offset_in_source_bytes": ("host/readv_plan.cc", "emit(q, take, 1, row * r.dst_pitch + col / ss * ds);",
                                              "emit(q, take, 1, row * r.dst_pitch + col / ss * (r.src_dtype == CV_DTYPE_F16 && r.dst_dtype == CV_DTYPE_F32 ? ss : ds));  /* planted */"),
     # the readv staging slots are spaced by the block length rounded down to 16 bytes: blocks whose length is not a multiple of 16
     # overlap their neighbour's slot
