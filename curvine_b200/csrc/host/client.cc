@@ -244,12 +244,28 @@ static Protocol request_proto(int8_t status, int64_t req_id, int32_t seq_id) {
     return p;
 }
 
-Err BlockClient::open_block(const ClientConf& conf, const ExtendedBlock& b, int64_t off, int64_t len, int64_t req_id, int32_t seq_id,
-                            bool short_circuit, int64_t chunk_size, BlockReadResponse* out, bool accept_arena) {
+// request frame -> the end of `out`
+static void append_frame(const Protocol& req, const std::string& header, std::string* out) {
+    Protocol p = req;
+    p.header_len = static_cast<int32_t>(header.size()), p.data_len = 0;
+    const size_t at = out->size();
+    out->resize(at + kProtocolSize);
+    encode_protocol(p, reinterpret_cast<uint8_t*>(&(*out)[at]));
+    out->append(header);
+}
+
+static BlockReadRequest open_request(const ClientConf& conf, const ExtendedBlock& b, int64_t off, int64_t len, bool short_circuit, int64_t chunk_size,
+                                     bool accept_arena) {
     BlockReadRequest r;
     r.id = b.id, r.off = off, r.len = len, r.chunk_size = static_cast<int32_t>(chunk_size), r.short_circuit = short_circuit;
     r.accept_arena = accept_arena && short_circuit;
     r.enable_read_ahead = conf.enable_read_ahead, r.read_ahead_len = conf.read_ahead_len, r.drop_cache_len = conf.drop_cache_len;
+    return r;
+}
+
+Err BlockClient::open_block(const ClientConf& conf, const ExtendedBlock& b, int64_t off, int64_t len, int64_t req_id, int32_t seq_id,
+                            bool short_circuit, int64_t chunk_size, BlockReadResponse* out, bool accept_arena) {
+    const BlockReadRequest r = open_request(conf, b, off, len, short_circuit, chunk_size, accept_arena);
     Protocol resp;
     std::string rh, rd;
     CV_RETURN_IF_ERR(rpc(request_proto(kReqOpen, req_id, seq_id), r.encode(), &resp, &rh, &rd));
@@ -273,20 +289,48 @@ Err BlockClient::read_commit_deferred(const ExtendedBlock& b, int64_t req_id, in
     return Err::ok();
 }
 
+Err BlockClient::open_blocks(const ClientConf& conf, const std::vector<OpenReq>& reqs, int64_t chunk_size, bool accept_arena,
+                             std::vector<BlockReadResponse>* out) {
+    std::string buf;
+    for (const OpenReq& q : reqs) append_frame(request_proto(kReqOpen, q.req_id, 0), open_request(conf, *q.b, q.off, q.b->len, true, chunk_size, accept_arena).encode(), &buf);
+    Err e = send_all(fd_, buf.data(), buf.size());
+    if (!e) e = drain_pending();  // the worker answers in order: the deferred Completes' answers come first
+    out->assign(reqs.size(), BlockReadResponse());
+    for (size_t i = 0; i < reqs.size() && !e; i++) {
+        Protocol resp;
+        std::string rh, rd;
+        e = recv_response_head(&resp, &rh);
+        if (!e && resp.data_len < 0) e = Err::common(str_printf("Invalid length %d", resp.data_len));
+        rd.resize(e ? 0 : static_cast<size_t>(resp.data_len));
+        if (!e && !rd.empty()) e = recv_exact(fd_, &rd[0], rd.size());
+        if (!e) e = check_echo(request_proto(kReqOpen, reqs[i].req_id, 0), resp);
+        if (!e && !resp.is_success()) e = decode_error_body(reinterpret_cast<const uint8_t*>(rd.data()), rd.size());
+        if (!e) e = BlockReadResponse::decode(reinterpret_cast<const uint8_t*>(rh.data()), rh.size(), &(*out)[i]);
+    }
+    if (e) broken = true;
+    return e;
+}
+
+Err BlockClient::read_commit_deferred(const std::vector<OpenReq>& reqs) {
+    std::string buf;
+    for (const OpenReq& q : reqs) {
+        BlockReadRequest r;
+        r.id = q.b->id;
+        append_frame(request_proto(kReqComplete, q.req_id, 1), r.encode(), &buf);
+    }
+    if (Err e = send_all(fd_, buf.data(), buf.size())) {
+        broken = true;
+        return e;
+    }
+    for (const OpenReq& q : reqs) pending_.push_back(request_proto(kReqComplete, q.req_id, 1));
+    return Err::ok();
+}
+
 Err BlockClient::send_block_read_pipeline(const ClientConf& conf, const ExtendedBlock& b, int64_t off, int64_t req_id, int64_t chunk_size, int64_t n_running,
                                           BlockReadResponse* open_resp) {
     if (!pending_.empty()) CV_RETURN_IF_ERR(drain_pending());
-    auto frame = [](const Protocol& req, const std::string& header, std::string* out) {
-        Protocol p = req;
-        p.header_len = static_cast<int32_t>(header.size()), p.data_len = 0;
-        const size_t at = out->size();
-        out->resize(at + kProtocolSize);
-        encode_protocol(p, reinterpret_cast<uint8_t*>(&(*out)[at]));
-        out->append(header);
-    };
-    BlockReadRequest r;
-    r.id = b.id, r.off = off, r.len = b.len, r.chunk_size = static_cast<int32_t>(chunk_size), r.short_circuit = false;
-    r.enable_read_ahead = conf.enable_read_ahead, r.read_ahead_len = conf.read_ahead_len, r.drop_cache_len = conf.drop_cache_len;
+    auto frame = append_frame;
+    const BlockReadRequest r = open_request(conf, b, off, b.len, false, chunk_size, false);
     std::string out;
     const Protocol open = request_proto(kReqOpen, req_id, 0);
     frame(open, r.encode(), &out);

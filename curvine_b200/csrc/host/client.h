@@ -101,6 +101,15 @@ class BlockClient {
     // Complete without waiting for the answer (GPU reader: one round trip less per block).  The response is consumed -- and its
     // echo / status checked -- before the next request goes out on this connection (drain_pending), also after a trip through the pool.
     Err read_commit_deferred(const ExtendedBlock& b, int64_t req_id, int32_t seq_id);
+    // Short-circuit Opens of several blocks in ONE write, then their answers in order (after those of the deferred Completes still
+    // owed); Completes (seq_id 1) of several blocks in one write, deferred.  Same messages and request ids as one call per block.  Any error leaves
+    // the connection broken: answers behind the failed one may still be on the wire.
+    struct OpenReq {
+        const ExtendedBlock* b;
+        int64_t off, req_id;
+    };
+    Err open_blocks(const ClientConf& conf, const std::vector<OpenReq>& reqs, int64_t chunk_size, bool accept_arena, std::vector<BlockReadResponse>* out);
+    Err read_commit_deferred(const std::vector<OpenReq>& reqs);
     Err drain_pending();
     size_t pending() const { return pending_.size(); }
     // Whole-block pipelining for the GPU reader's framed path: Open, every Running request and the Complete of one block leave in

@@ -848,12 +848,17 @@ struct GpuFsReader::Call {
         std::vector<int64_t> lens(n), rids(n), base_offs(n, 0);
         size_t n_arena = 0;
         Err e;
-        for (size_t i = 0; i < n && !e; i++) {
-            const Job& job = jobs[gr.j0 + i];
-            BlockReadResponse resp;
-            e = open_short_circuit(r.ctx_, *job.lb, job.block_off, conn, &rids[i], &resp);
-            paths[i] = resp.path, lens[i] = job.lb->block.len;
-            if (resp.has_arena) base_offs[i] = resp.arena_off, n_arena++;
+        std::vector<BlockReadResponse> resps;
+        if (!open_group_batched(gr, conn, &rids, &resps)) {  // one Open round trip per block, with failover to the other replicas
+            resps.assign(n, BlockReadResponse());
+            for (size_t i = 0; i < n && !e; i++) {
+                const Job& job = jobs[gr.j0 + i];
+                e = open_short_circuit(r.ctx_, *job.lb, job.block_off, conn, &rids[i], &resps[i]);
+            }
+        }
+        for (size_t i = 0; i < n; i++) {
+            paths[i] = resps[i].path, lens[i] = jobs[gr.j0 + i].lb->block.len;
+            if (resps[i].has_arena) base_offs[i] = resps[i].arena_off, n_arena++;
         }
         bool via_ring = n_arena > 0;  // arena extents (mixed group, or segments that cannot be pinned): pread out of the segment file
         if (!e && n_arena == n && !G.arena.unsupported.load(std::memory_order_relaxed)) {
@@ -889,6 +894,30 @@ struct GpuFsReader::Call {
         return e ? e : copy_err;
     }
 
+    // The group's Opens in one write and one round trip, on a connection to the first replica of its blocks when they all share it.
+    // false: not done (blocks on different first replicas, no connection, an error or a block file the worker did not name): the
+    // connection is broken if anything was sent, and the per-block path redoes the Opens on a fresh one, failover included.
+    bool open_group_batched(const Group& gr, std::unique_ptr<BlockClient>* conn, std::vector<int64_t>* rids, std::vector<BlockReadResponse>* resps) {
+        const WorkerAddress& a = jobs[gr.j0].lb->locs[0];  // plain jobs have a replica
+        std::vector<BlockClient::OpenReq> reqs;
+        for (size_t j = gr.j0; j < gr.j1; j++) {
+            if (!(jobs[j].lb->locs[0] == a)) return false;
+            reqs.push_back(BlockClient::OpenReq{&jobs[j].lb->block, jobs[j].block_off, new_req_id()});
+        }
+        if (!*conn || !((*conn)->addr() == a) || (*conn)->broken) {
+            if (*conn) r.ctx_->release(std::move(*conn));
+            if (r.ctx_->acquire_read(a, conn)) return false;
+        }
+        if ((*conn)->open_blocks(r.ctx_->conf.client, reqs, r.ctx_->read_chunk_size(), r.ctx_->conf.b200.arena, resps)) return false;
+        for (const BlockReadResponse& x : *resps)
+            if (!x.has_path) {
+                (*conn)->broken = true;  // the per-block path reports it ("read_context.path is none") or fails over
+                return false;
+            }
+        for (size_t i = 0; i < reqs.size(); i++) (*rids)[i] = reqs[i].req_id;
+        return true;
+    }
+
     // Every block of the group is an extent of an arena segment this context pinned once.  kUnsupported: a segment cannot be pinned.
     Err fetch_arena(const Group& gr, const std::vector<std::string>& paths, const std::vector<int64_t>& base_offs, const std::vector<int64_t>& rids,
                     std::unique_ptr<BlockClient>* conn) {
@@ -905,8 +934,9 @@ struct GpuFsReader::Call {
             q.add(d_dst + job.dst_off, segs[i]->base + base_offs[i] + job.block_off, static_cast<size_t>(job.n), segs[i].get());
         }
         const Err copy_err = q.finish();
-        Err e;
-        for (size_t j = gr.j0; j < gr.j1 && !e; j++) e = (*conn)->read_commit_deferred(jobs[j].lb->block, rids[j - gr.j0], 1);
+        std::vector<BlockClient::OpenReq> done;  // the group's Completes in one write, answered in front of the next request
+        for (size_t j = gr.j0; j < gr.j1; j++) done.push_back(BlockClient::OpenReq{&jobs[j].lb->block, jobs[j].block_off, rids[j - gr.j0]});
+        const Err e = (*conn)->read_commit_deferred(done);
         if (e || copy_err) return e ? e : copy_err;
         G.arena.dma_jobs += gr.j1 - gr.j0;
         for (size_t j = gr.j0; j < gr.j1; j++) G.arena.dma_bytes += static_cast<uint64_t>(jobs[j].n);
