@@ -58,6 +58,19 @@ struct Err {
         if (e__) return e__;        \
     } while (0)
 
+// A failed CUDA runtime call (CU_TRY) or cvk_* launcher (CVK_TRY) returns Err::io naming the call.  They name no CUDA type until they
+// expand, so CUDA-free modules can include this header.
+#define CU_TRY(x)                                                                                              \
+    do {                                                                                                       \
+        cudaError_t e_ = (x);                                                                                  \
+        if (e_ != cudaSuccess) return ::cv::Err::io(::cv::str_printf("%s: %s", #x, cudaGetErrorString(e_)));  \
+    } while (0)
+#define CVK_TRY(x)                                                                                             \
+    do {                                                                                                       \
+        int e_ = (x);                                                                                          \
+        if (e_ != 0) return ::cv::Err::io(::cv::str_printf("%s: %s", #x, cudaGetErrorString(cudaError_t(e_)))); \
+    } while (0)
+
 inline void put_be32(uint8_t* p, uint32_t v) { p[0] = v >> 24, p[1] = v >> 16, p[2] = v >> 8, p[3] = v; }
 inline void put_be64(uint8_t* p, uint64_t v) {
     put_be32(p, static_cast<uint32_t>(v >> 32));

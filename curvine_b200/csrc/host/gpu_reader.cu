@@ -18,17 +18,6 @@
 
 namespace cv {
 
-#define CU_TRY(x)                                                                                   \
-    do {                                                                                            \
-        cudaError_t e_ = (x);                                                                       \
-        if (e_ != cudaSuccess) return Err::io(str_printf("%s: %s", #x, cudaGetErrorString(e_)));    \
-    } while (0)
-#define CVK_TRY(x)                                                                                  \
-    do {                                                                                            \
-        int e_ = (x);                                                                               \
-        if (e_ != 0) return Err::io(str_printf("%s: %s", #x, cudaGetErrorString(cudaError_t(e_)))); \
-    } while (0)
-
 // ------------------------------------------------------------------ GpuIngest: ring + streams
 
 class GpuIngest {

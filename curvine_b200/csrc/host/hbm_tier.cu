@@ -4,20 +4,9 @@
 
 #include <vector>
 
-#include "../../../include/curvine_b200_kernels.h"
 #include "wire.h"
 
 namespace cv {
-
-#define CUH_TRY(x)                                                                               \
-    do {                                                                                         \
-        cudaError_t e_ = (x);                                                                    \
-        if (e_ != cudaSuccess) return Err::io(str_printf("%s: %s", #x, cudaGetErrorString(e_))); \
-    } while (0)
-
-PackedStream::~PackedStream() {
-    if (wire) cudaFreeHost(wire);
-}
 
 HbmBuf::~HbmBuf() {
     if (!d_ptr) return;
@@ -176,45 +165,14 @@ void HbmTier::stats(int64_t out[6]) const {
 
 Err HbmTier::pack(const HbmBlock& blk, int64_t off, int64_t n, int64_t chunk, int64_t req_id, int32_t first_seq, PackedStream* out) const {
     const HbmBuf& b = *blk;
-    CUH_TRY(cudaSetDevice(b.device));
-    const uint32_t nf = static_cast<uint32_t>((n + chunk - 1) / chunk);
-    const size_t wire_bytes = static_cast<size_t>(n) + size_t(nf) * kProtocolSize;
-    if (wire_bytes > out->wire_cap) {
-        if (out->wire) cudaFreeHost(out->wire);
-        out->wire = nullptr;
-        CUH_TRY(cudaHostAlloc(&out->wire, wire_bytes, cudaHostAllocDefault));
-        out->wire_cap = wire_bytes;
-    }
+    CU_TRY(cudaSetDevice(b.device));
     out->off0 = off, out->total = n, out->chunk = chunk, out->req_id = req_id, out->first_seq = first_seq;
-    if (nf == 0) return Err::ok();
-    std::vector<CvFrameDesc> descs(nf);
-    for (uint32_t f = 0; f < nf; f++) {
-        CvFrameDesc& d = descs[f];
-        memset(&d, 0, sizeof(d));
-        d.wire_off = uint64_t(f) * (kProtocolSize + chunk);
-        d.dst_off = static_cast<uint64_t>(off) + uint64_t(f) * chunk;  // source offset inside the resident block
-        d.data_len = static_cast<uint32_t>(std::min<int64_t>(chunk, n - int64_t(f) * chunk));
-        d.req_id = req_id, d.seq_id = first_seq + static_cast<int32_t>(f), d.block = 0, d.code = kCodeReadBlock;
-        d.status = static_cast<uint8_t>(status_encode(kReqRunning, kRespSuccess));  // 0x03
-    }
     cudaStream_t st;
-    CUH_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    uint8_t* d_buf = nullptr;
-    const size_t o_desc = (wire_bytes + 255) & ~size_t(255), o_crc = o_desc + sizeof(CvFrameDesc) * nf;
-    Err err;
-    cudaError_t ce = cudaMallocAsync(&d_buf, o_crc + 64, st);
-    if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_buf + o_desc, descs.data(), sizeof(CvFrameDesc) * nf, cudaMemcpyHostToDevice, st);
-    int rc = ce != cudaSuccess ? int(ce)
-                               : cvk_pack_frames(b.d_ptr, reinterpret_cast<const CvFrameDesc*>(d_buf + o_desc), nf, 1, d_buf, CV_POLY_CASTAGNOLI,
-                                                 static_cast<uint64_t>(n), reinterpret_cast<uint32_t*>(d_buf + o_crc), st);
-    if (!rc) ce = cudaMemcpyAsync(out->wire, d_buf, wire_bytes, cudaMemcpyDeviceToHost, st);
-    if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(&out->crc32c, d_buf + o_crc, 4, cudaMemcpyDeviceToHost, st);
-    if (d_buf) cudaFreeAsync(d_buf, st);
-    if (!rc && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+    CU_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    Err e = pack_running_frames(b.d_ptr + off, n, chunk, kCodeReadBlock, static_cast<uint8_t>(status_encode(kReqRunning, kRespSuccess)), req_id,
+                                first_seq, st, out);
     cudaStreamDestroy(st);
-    if (rc) return Err::io(str_printf("cvk_pack_frames: %s", cudaGetErrorString(cudaError_t(rc))));
-    if (ce != cudaSuccess) return Err::io(str_printf("hbm pack: %s", cudaGetErrorString(ce)));
-    return Err::ok();
+    return e;
 }
 
 }  // namespace cv

@@ -19,6 +19,7 @@
 #include <unordered_map>
 
 #include "common.h"
+#include "packed_frames.h"
 
 namespace cv {
 
@@ -32,17 +33,6 @@ struct HbmBuf {
     ~HbmBuf();
 };
 using HbmBlock = std::shared_ptr<const HbmBuf>;
-
-// The packed response stream of one block read: frame f = wire + f*(22+chunk), carries min(chunk, remaining) bytes.
-struct PackedStream {
-    uint8_t* wire = nullptr;  // pinned host memory
-    size_t wire_cap = 0;
-    int64_t off0 = 0, total = 0, chunk = 0;
-    int64_t req_id = 0;
-    int32_t first_seq = 1;
-    uint32_t crc32c = 0;  // CRC-32C of the packed payload, computed at the source by K4
-    ~PackedStream();
-};
 
 // Admission / eviction (the tier sits beside Mem/Ssd/Hdd; the reference's tiers are capacity-bounded directories chosen by
 // storage policy, worker/storage/policy.rs:56-105 -- here the policy is LRU over resident blocks):

@@ -1,7 +1,5 @@
 #include "writer.h"
 
-#include <cuda_runtime.h>
-
 #include "../../../include/curvine_b200.h"
 #include "../crc_gf.h"
 #include "block_store.h"
@@ -16,7 +14,6 @@ uint32_t host_crc_update(int poly, uint32_t crc, const uint8_t* buf, size_t len)
 }
 
 FsWriter::~FsWriter() {
-    if (h_wire_) cudaFreeHost(h_wire_);
     if (client_) ctx_->release(std::move(client_));
 }
 
@@ -114,15 +111,8 @@ Err FsWriter::write(const uint8_t* buf, int64_t n) {
     return Err::ok();
 }
 
-#define CUW_TRY(x)                                                                               \
-    do {                                                                                         \
-        cudaError_t e_ = (x);                                                                    \
-        if (e_ != cudaSuccess) return Err::io(str_printf("%s: %s", #x, cudaGetErrorString(e_))); \
-    } while (0)
-
 Err FsWriter::write_device(const void* d_src, int64_t n, void* stream) {
     if (done_) return Err::common("writer is closed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
     const uint8_t* src = static_cast<const uint8_t*>(d_src);
     while (n > 0) {
         if (block_open_ && block_pos_ == block_size_) CV_RETURN_IF_ERR(commit_block(false));
@@ -130,40 +120,11 @@ Err FsWriter::write_device(const void* d_src, int64_t n, void* stream) {
         const int64_t take = std::min(n, block_size_ - block_pos_);  // the rest of this block in one K4 launch
         const uint32_t nf = static_cast<uint32_t>((take + chunk_size_ - 1) / chunk_size_);
         const size_t wire_bytes = static_cast<size_t>(take) + size_t(nf) * kProtocolSize;
-        if (wire_bytes > h_wire_cap_) {
-            if (h_wire_) cudaFreeHost(h_wire_);
-            h_wire_cap_ = wire_bytes;
-            CUW_TRY(cudaHostAlloc(&h_wire_, h_wire_cap_, cudaHostAllocDefault));
-        }
-        std::vector<CvFrameDesc> descs(nf);
-        for (uint32_t f = 0; f < nf; f++) {
-            CvFrameDesc& d = descs[f];
-            memset(&d, 0, sizeof(d));
-            d.wire_off = uint64_t(f) * (kProtocolSize + chunk_size_);
-            d.dst_off = uint64_t(f) * chunk_size_;  // offset of this chunk inside the source range
-            d.data_len = static_cast<uint32_t>(std::min<int64_t>(chunk_size_, take - int64_t(f) * chunk_size_));
-            d.req_id = req_id_, d.seq_id = seq_ + 1 + static_cast<int32_t>(f), d.block = 0, d.code = kCodeWriteBlock;
-            d.status = static_cast<uint8_t>(status_encode(kReqRunning, kRespUndefined));  // 0xF3
-        }
-        uint8_t* d_buf = nullptr;  // [wire image][descs][crc32c][off,len][crc32]
-        const size_t o_desc = (wire_bytes + 255) & ~size_t(255), o_crc = o_desc + sizeof(CvFrameDesc) * nf, o_tab = (o_crc + 4 + 255) & ~size_t(255);
-        CUW_TRY(cudaMallocAsync(&d_buf, o_tab + 64, st));
-        CUW_TRY(cudaMemcpyAsync(d_buf + o_desc, descs.data(), sizeof(CvFrameDesc) * nf, cudaMemcpyHostToDevice, st));
-        const uint64_t tab[2] = {0, static_cast<uint64_t>(take)};
-        CUW_TRY(cudaMemcpyAsync(d_buf + o_tab, tab, sizeof(tab), cudaMemcpyHostToDevice, st));
-        int rc = cvk_pack_frames(src, reinterpret_cast<const CvFrameDesc*>(d_buf + o_desc), nf, 1, d_buf, CV_POLY_CASTAGNOLI, static_cast<uint64_t>(take),
-                                 reinterpret_cast<uint32_t*>(d_buf + o_crc), stream);
-        if (!rc) rc = cvk_crc_blocks(src, reinterpret_cast<const uint64_t*>(d_buf + o_tab), reinterpret_cast<const uint64_t*>(d_buf + o_tab + 8), 1,
-                                     CV_POLY_IEEE, static_cast<uint64_t>(take), reinterpret_cast<uint32_t*>(d_buf + o_tab + 16), stream);
-        if (rc) return Err::io(str_printf("cvk_pack_frames: %s", cudaGetErrorString(cudaError_t(rc))));
-        uint32_t crcs[2] = {0, 0};
-        CUW_TRY(cudaMemcpyAsync(h_wire_, d_buf, wire_bytes, cudaMemcpyDeviceToHost, st));
-        CUW_TRY(cudaMemcpyAsync(&crcs[0], d_buf + o_crc, 4, cudaMemcpyDeviceToHost, st));
-        CUW_TRY(cudaMemcpyAsync(&crcs[1], d_buf + o_tab + 16, 4, cudaMemcpyDeviceToHost, st));
-        CUW_TRY(cudaFreeAsync(d_buf, st));
-        CUW_TRY(cudaStreamSynchronize(st));
+        uint32_t crc32 = 0;
+        CV_RETURN_IF_ERR(pack_running_frames(src, take, chunk_size_, kCodeWriteBlock, static_cast<uint8_t>(status_encode(kReqRunning, kRespUndefined)),
+                                             req_id_, seq_ + 1, stream, &packed_, &crc32));
         // all Running frames of this range in one write, then their responses (the worker serves them in order)
-        Err e = send_all(client_->fd(), h_wire_, wire_bytes);
+        Err e = send_all(client_->fd(), packed_.wire, wire_bytes);
         for (uint32_t f = 0; f < nf && !e; f++) {
             Protocol resp;
             std::string rh;
@@ -178,8 +139,8 @@ Err FsWriter::write_device(const void* d_src, int64_t n, void* stream) {
             return e;
         }
         seq_ += static_cast<int32_t>(nf);
-        crc32c_ = crc_combine(crc32c_, crcs[0], static_cast<uint64_t>(take), kPolyCastagnoli);
-        crc32_ = crc_combine(crc32_, crcs[1], static_cast<uint64_t>(take), kPolyIeee);
+        crc32c_ = crc_combine(crc32c_, packed_.crc32c, static_cast<uint64_t>(take), kPolyCastagnoli);
+        crc32_ = crc_combine(crc32_, crc32, static_cast<uint64_t>(take), kPolyIeee);
         src += take, n -= take, block_pos_ += take, pos_ += take;
     }
     return Err::ok();

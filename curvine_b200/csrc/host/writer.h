@@ -11,6 +11,7 @@
 // the payload behind them while CRC-ing the source, the wire image goes D2H once and onto the socket verbatim.
 #pragma once
 #include "client.h"
+#include "packed_frames.h"
 
 namespace cv {
 
@@ -41,8 +42,7 @@ class FsWriter {
     int64_t block_pos_ = 0, req_id_ = 0;
     int32_t seq_ = 0;
     uint32_t crc32_ = 0, crc32c_ = 0;  // running CRCs of the open block
-    uint8_t* h_wire_ = nullptr;
-    size_t h_wire_cap_ = 0;
+    PackedStream packed_;  // write_device's wire image, reused from call to call
     bool done_ = false;
 };
 
