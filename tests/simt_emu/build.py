@@ -200,6 +200,20 @@ MUTATIONS = {
     # overlap their neighbour's slot
     "readv_stage_slots_rounded_down_to_16": ("host/gpu_reader.cu", "const int64_t at = rel(stage + slot * static_cast<size_t>(stage_block));",
                                              "const int64_t at = rel(stage + slot * static_cast<size_t>(stage_block & ~int64_t(15)));  /* planted */"),
+    # K2's prefix checks (tests/test_kernel_verdicts_mutants.py): a frame of another RPC, of another request, or with a header in front
+    # of its payload is accepted; a legal 16 MiB frame is rejected
+    "k2_ignores_header_len": ("kernels.cu", "if (header_len != static_cast<int32_t>(d.header_len)) e |= CV_FERR_HEADER_LEN;", "/* planted: no header_len check */"),
+    "k2_ignores_code": ("kernels.cu", "if (code != d.code) e |= CV_FERR_CODE;", "/* planted: no code check */"),
+    "k2_ignores_total_len": ("kernels.cu", "if (int64_t(total_len) != int64_t(CV_HEAD_SIZE) + d.header_len + d.data_len) e |= CV_FERR_TOTAL_LEN;",
+                             "/* planted: no total_len check */"),
+    "k2_compares_req_id_low_words": ("kernels.cu", "if (req_id != d.req_id) e |= CV_FERR_REQ_ID;",
+                                     "if (uint32_t(req_id) != uint32_t(d.req_id)) e |= CV_FERR_REQ_ID;  /* planted */"),
+    "k2_rejects_16_mib_of_data": ("kernels.cu", "data_len > CV_MAX_DATA_SIZE) e |= CV_FERR_DATA_RANGE;", "data_len >= CV_MAX_DATA_SIZE) e |= CV_FERR_DATA_RANGE;  /* planted */"),
+    # cvk_verify_crcs / _masked: one count per warp with a mismatch, skipped entries compared, a mask entry never cleared
+    "verify_counts_warps": ("kernels.cu", "atomicAdd(n_bad, __popc(m));", "atomicAdd(n_bad, 1u);  /* planted */"),
+    "verify_ignores_the_skip_mask": ("kernels.cu", "const bool bad = i < n && !(skip && skip[i]) && crc[i] != expect[i];",
+                                     "const bool bad = i < n && crc[i] != expect[i];  /* planted */"),
+    "verify_marks_only_mismatches": ("kernels.cu", "if (i < n && bad_mask) bad_mask[i] = bad;", "if (i < n && bad_mask && bad) bad_mask[i] = 1;  /* planted */"),
 }
 
 
