@@ -149,109 +149,61 @@ Err Namespace::get_block_locations(const std::string& path, std::shared_ptr<cons
 
 BlockClient::~BlockClient() { close_fd(fd_); }
 
-static Protocol request_proto(int8_t status, int64_t req_id, int32_t seq_id);
-
 Err BlockClient::drain_pending() {
+    Protocol resp;
+    std::string rh, rd;
     while (!pending_.empty()) {
         const Protocol req = pending_.front();
         pending_.erase(pending_.begin());
-        Protocol resp;
-        std::string rh, rd;
-        CV_RETURN_IF_ERR(recv_response_head(&resp, &rh));
-        rd.resize(static_cast<size_t>(resp.data_len));
-        if (resp.data_len) {
-            Err e = recv_exact(fd_, &rd[0], rd.size());
-            if (e) {
-                broken = true;
-                return e;
-            }
-        }
-        if (req.req_id != resp.req_id || req.seq_id != resp.seq_id) {
-            broken = true;
-            return Err::common("response mismatch on a deferred Complete");
-        }
-        if (!resp.is_success()) return decode_error_body(reinterpret_cast<const uint8_t*>(rd.data()), rd.size());
+        CV_RETURN_IF_ERR(recv_answer(req, &resp, &rh, &rd));
     }
     return Err::ok();
 }
 
-Err BlockClient::send_request(const Protocol& req, const std::string& header) {
-    if (!pending_.empty()) CV_RETURN_IF_ERR(drain_pending());
+void BlockClient::append_frame(const Protocol& req, const std::string& header, std::string* out, int32_t data_len) {
     Protocol p = req;
-    p.header_len = static_cast<int32_t>(header.size());
-    p.data_len = 0;
-    std::string out(kProtocolSize, '\0');
-    encode_protocol(p, reinterpret_cast<uint8_t*>(&out[0]));
-    out += header;
+    p.header_len = static_cast<int32_t>(header.size()), p.data_len = data_len;
+    const size_t at = out->size();
+    out->resize(at + kProtocolSize);
+    encode_protocol(p, reinterpret_cast<uint8_t*>(&(*out)[at]));
+    out->append(header);
+}
+
+Err BlockClient::send_request(const Protocol& req, const std::string& header) {
+    CV_RETURN_IF_ERR(drain_pending());
+    std::string out;
+    append_frame(req, header, &out);
     Err e = send_all(fd_, out.data(), out.size());
     if (e) broken = true;
     return e;
 }
 
-Err BlockClient::recv_response_head(Protocol* resp, std::string* resp_header) {
+Err BlockClient::recv_answer(const Protocol& req, Protocol* resp, std::string* header, std::string* data) {
     uint8_t prefix[kProtocolSize];
-    for (;;) {
-        Err e = recv_exact(fd_, prefix, kProtocolSize);
+    Err e;
+    do {  // heartbeats are read whole and skipped (rpc_frame.rs:255-259)
+        e = recv_exact(fd_, prefix, kProtocolSize);
         if (!e) e = decode_protocol(prefix, resp);
         if (!e && resp->header_len < 0) e = Err::common(str_printf("Invalid length %d", resp->header_len));
-        if (e) {
-            broken = true;
-            return e;
-        }
-        resp_header->resize(static_cast<size_t>(resp->header_len));
-        if (resp->header_len && (e = recv_exact(fd_, &(*resp_header)[0], resp_header->size()))) {
-            broken = true;
-            return e;
-        }
-        if (!resp->is_heartbeat()) return Err::ok();
-        std::string skip(static_cast<size_t>(resp->data_len), '\0');  // rpc_frame.rs:255-259
-        if (resp->data_len && (e = recv_exact(fd_, &skip[0], skip.size()))) {
-            broken = true;
-            return e;
-        }
+        if (e) break;
+        header->resize(static_cast<size_t>(resp->header_len));
+        data->resize(static_cast<size_t>(resp->data_len));
+        if (resp->header_len) e = recv_exact(fd_, &(*header)[0], header->size());
+        if (!e && resp->data_len) e = recv_exact(fd_, &(*data)[0], data->size());
+    } while (!e && resp->is_heartbeat());
+    if (!e && (req.req_id != resp->req_id || req.seq_id != resp->seq_id))  // raw_client.rs:100-116
+        e = Err::common(str_printf("response mismatch: request (req_id %lld, seq_id %d), response (req_id %lld, seq_id %d)", (long long)req.req_id,
+                                   req.seq_id, (long long)resp->req_id, resp->seq_id));
+    if (e) {
+        broken = true;
+        return e;
     }
-}
-
-static Err check_echo(const Protocol& req, const Protocol& resp) {  // raw_client.rs:100-116
-    if (req.req_id != resp.req_id || req.seq_id != resp.seq_id)
-        return Err::common(str_printf("response mismatch: request (req_id %lld, seq_id %d), response (req_id %lld, seq_id %d)", (long long)req.req_id,
-                                      req.seq_id, (long long)resp.req_id, resp.seq_id));
-    return Err::ok();
+    return resp->is_success() ? Err::ok() : decode_error_body(reinterpret_cast<const uint8_t*>(data->data()), data->size());
 }
 
 Err BlockClient::rpc(const Protocol& req, const std::string& header, Protocol* resp, std::string* resp_header, std::string* resp_data) {
     CV_RETURN_IF_ERR(send_request(req, header));
-    CV_RETURN_IF_ERR(recv_response_head(resp, resp_header));
-    resp_data->resize(static_cast<size_t>(resp->data_len));
-    if (resp->data_len) {
-        Err e = recv_exact(fd_, &(*resp_data)[0], resp_data->size());
-        if (e) {
-            broken = true;
-            return e;
-        }
-    }
-    if (Err e = check_echo(req, *resp)) {
-        broken = true;
-        return e;
-    }
-    if (!resp->is_success()) return decode_error_body(reinterpret_cast<const uint8_t*>(resp_data->data()), resp_data->size());
-    return Err::ok();
-}
-
-static Protocol request_proto(int8_t status, int64_t req_id, int32_t seq_id) {
-    Protocol p;
-    p.code = kCodeReadBlock, p.req_status = status, p.resp_status = kRespUndefined, p.req_id = req_id, p.seq_id = seq_id;
-    return p;
-}
-
-// request frame -> the end of `out`
-static void append_frame(const Protocol& req, const std::string& header, std::string* out) {
-    Protocol p = req;
-    p.header_len = static_cast<int32_t>(header.size()), p.data_len = 0;
-    const size_t at = out->size();
-    out->resize(at + kProtocolSize);
-    encode_protocol(p, reinterpret_cast<uint8_t*>(&(*out)[at]));
-    out->append(header);
+    return recv_answer(req, resp, resp_header, resp_data);
 }
 
 static BlockReadRequest open_request(const ClientConf& conf, const ExtendedBlock& b, int64_t off, int64_t len, bool short_circuit, int64_t chunk_size,
@@ -268,7 +220,7 @@ Err BlockClient::open_block(const ClientConf& conf, const ExtendedBlock& b, int6
     const BlockReadRequest r = open_request(conf, b, off, len, short_circuit, chunk_size, accept_arena);
     Protocol resp;
     std::string rh, rd;
-    CV_RETURN_IF_ERR(rpc(request_proto(kReqOpen, req_id, seq_id), r.encode(), &resp, &rh, &rd));
+    CV_RETURN_IF_ERR(rpc(request_proto(kCodeReadBlock, kReqOpen, req_id, seq_id), r.encode(), &resp, &rh, &rd));
     return BlockReadResponse::decode(reinterpret_cast<const uint8_t*>(rh.data()), rh.size(), out);
 }
 
@@ -277,13 +229,13 @@ Err BlockClient::read_commit(const ExtendedBlock& b, int64_t req_id, int32_t seq
     r.id = b.id;
     Protocol resp;
     std::string rh, rd;
-    return rpc(request_proto(kReqComplete, req_id, seq_id), r.encode(), &resp, &rh, &rd);
+    return rpc(request_proto(kCodeReadBlock, kReqComplete, req_id, seq_id), r.encode(), &resp, &rh, &rd);
 }
 
 Err BlockClient::read_commit_deferred(const ExtendedBlock& b, int64_t req_id, int32_t seq_id) {
     BlockReadRequest r;
     r.id = b.id;
-    const Protocol p = request_proto(kReqComplete, req_id, seq_id);
+    const Protocol p = request_proto(kCodeReadBlock, kReqComplete, req_id, seq_id);
     CV_RETURN_IF_ERR(send_request(p, r.encode()));
     pending_.push_back(p);
     return Err::ok();
@@ -292,19 +244,15 @@ Err BlockClient::read_commit_deferred(const ExtendedBlock& b, int64_t req_id, in
 Err BlockClient::open_blocks(const ClientConf& conf, const std::vector<OpenReq>& reqs, int64_t chunk_size, bool accept_arena,
                              std::vector<BlockReadResponse>* out) {
     std::string buf;
-    for (const OpenReq& q : reqs) append_frame(request_proto(kReqOpen, q.req_id, 0), open_request(conf, *q.b, q.off, q.b->len, true, chunk_size, accept_arena).encode(), &buf);
+    for (const OpenReq& q : reqs)
+        append_frame(request_proto(kCodeReadBlock, kReqOpen, q.req_id, 0), open_request(conf, *q.b, q.off, q.b->len, true, chunk_size, accept_arena).encode(), &buf);
     Err e = send_all(fd_, buf.data(), buf.size());
     if (!e) e = drain_pending();  // the worker answers in order: the deferred Completes' answers come first
     out->assign(reqs.size(), BlockReadResponse());
+    Protocol resp;
+    std::string rh, rd;
     for (size_t i = 0; i < reqs.size() && !e; i++) {
-        Protocol resp;
-        std::string rh, rd;
-        e = recv_response_head(&resp, &rh);
-        if (!e && resp.data_len < 0) e = Err::common(str_printf("Invalid length %d", resp.data_len));
-        rd.resize(e ? 0 : static_cast<size_t>(resp.data_len));
-        if (!e && !rd.empty()) e = recv_exact(fd_, &rd[0], rd.size());
-        if (!e) e = check_echo(request_proto(kReqOpen, reqs[i].req_id, 0), resp);
-        if (!e && !resp.is_success()) e = decode_error_body(reinterpret_cast<const uint8_t*>(rd.data()), rd.size());
+        e = recv_answer(request_proto(kCodeReadBlock, kReqOpen, reqs[i].req_id, 0), &resp, &rh, &rd);
         if (!e) e = BlockReadResponse::decode(reinterpret_cast<const uint8_t*>(rh.data()), rh.size(), &(*out)[i]);
     }
     if (e) broken = true;
@@ -316,52 +264,39 @@ Err BlockClient::read_commit_deferred(const std::vector<OpenReq>& reqs) {
     for (const OpenReq& q : reqs) {
         BlockReadRequest r;
         r.id = q.b->id;
-        append_frame(request_proto(kReqComplete, q.req_id, 1), r.encode(), &buf);
+        append_frame(request_proto(kCodeReadBlock, kReqComplete, q.req_id, 1), r.encode(), &buf);
     }
     if (Err e = send_all(fd_, buf.data(), buf.size())) {
         broken = true;
         return e;
     }
-    for (const OpenReq& q : reqs) pending_.push_back(request_proto(kReqComplete, q.req_id, 1));
+    for (const OpenReq& q : reqs) pending_.push_back(request_proto(kCodeReadBlock, kReqComplete, q.req_id, 1));
     return Err::ok();
 }
 
 Err BlockClient::send_block_read_pipeline(const ClientConf& conf, const ExtendedBlock& b, int64_t off, int64_t req_id, int64_t chunk_size, int64_t n_running,
                                           BlockReadResponse* open_resp) {
-    if (!pending_.empty()) CV_RETURN_IF_ERR(drain_pending());
-    auto frame = append_frame;
+    CV_RETURN_IF_ERR(drain_pending());
     const BlockReadRequest r = open_request(conf, b, off, b.len, false, chunk_size, false);
     std::string out;
-    const Protocol open = request_proto(kReqOpen, req_id, 0);
-    frame(open, r.encode(), &out);
-    for (int64_t f = 0; f < n_running; f++) frame(request_proto(kReqRunning, req_id, static_cast<int32_t>(f + 1)), std::string(), &out);
+    const Protocol open = request_proto(kCodeReadBlock, kReqOpen, req_id, 0);
+    append_frame(open, r.encode(), &out);
+    for (int64_t f = 0; f < n_running; f++) append_frame(request_proto(kCodeReadBlock, kReqRunning, req_id, static_cast<int32_t>(f + 1)), std::string(), &out);
     BlockReadRequest c;  // ..Default::default() but the id (block_client.rs:263-266)
     c.id = b.id;
-    const Protocol complete = request_proto(kReqComplete, req_id, static_cast<int32_t>(n_running + 1));
-    frame(complete, c.encode(), &out);
-    if (Err e = send_all(fd_, out.data(), out.size())) {
-        broken = true;
-        return e;
-    }
+    const Protocol complete = request_proto(kCodeReadBlock, kReqComplete, req_id, static_cast<int32_t>(n_running + 1));
+    append_frame(complete, c.encode(), &out);
     Protocol resp;
     std::string rh, rd;
-    CV_RETURN_IF_ERR(recv_response_head(&resp, &rh));
-    rd.resize(static_cast<size_t>(resp.data_len));
-    if (resp.data_len)
-        if (Err e = recv_exact(fd_, &rd[0], rd.size())) {
-            broken = true;
-            return e;
-        }
-    if (Err e = check_echo(open, resp)) {
-        broken = true;
+    Err e = send_all(fd_, out.data(), out.size());
+    if (!e) e = recv_answer(open, &resp, &rh, &rd);
+    if (!e) e = BlockReadResponse::decode(reinterpret_cast<const uint8_t*>(rh.data()), rh.size(), open_resp);
+    if (e) {
+        broken = true;  // the answers to the requests already sent behind the Open are dropped with the connection
         return e;
     }
-    if (!resp.is_success()) {
-        broken = true;  // the answers to the requests already sent behind the Open are dropped with the connection
-        return decode_error_body(reinterpret_cast<const uint8_t*>(rd.data()), rd.size());
-    }
     pending_.push_back(complete);
-    return BlockReadResponse::decode(reinterpret_cast<const uint8_t*>(rh.data()), rh.size(), open_resp);
+    return Err::ok();
 }
 
 // ------------------------------------------------------------------ FsContext (connection pool)
@@ -426,6 +361,12 @@ void FsContext::release(std::unique_ptr<BlockClient> c) {
     c->idle_since_ms = now_ms();
     idle_[c->addr().str()].push_back(std::move(c));
     idle_total_++;
+}
+
+Err FsContext::connection_to(const WorkerAddress& addr, std::unique_ptr<BlockClient>* conn) {
+    if (*conn && (*conn)->addr() == addr && !(*conn)->broken) return Err::ok();
+    release(std::move(*conn));
+    return acquire_read(addr, conn);
 }
 
 void FsContext::add_failed_worker(const WorkerAddress& addr) {
@@ -583,7 +524,7 @@ Err BlockReader::read_once(std::string* buf) {
             }
             Protocol resp;
             std::string rh;
-            CV_RETURN_IF_ERR(client_->rpc(request_proto(kReqRunning, req_id_, ++seq_id_), header, &resp, &rh, buf));
+            CV_RETURN_IF_ERR(client_->rpc(request_proto(kCodeReadBlock, kReqRunning, req_id_, ++seq_id_), header, &resp, &rh, buf));
             break;
         }
     }

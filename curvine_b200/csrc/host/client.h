@@ -87,14 +87,24 @@ class Namespace {
 
 // ------------------------------------------------------------------ block RPC client
 
+// Every answer is read by recv_answer, and one rule decides whether the connection can still be used: any failure to send a request or
+// to receive, frame or match (request and seq id) its answer marks it `broken`, and FsContext::release closes it instead of pooling it.  A
+// well-formed error answer leaves it in step: the call returns the worker's error and the connection stays usable.  A call that has
+// already sent more requests behind the failed one (open_blocks, send_block_read_pipeline, FsWriter::write_device) marks it broken on
+// any error, since those answers may still be on the wire.
 class BlockClient {
    public:
     BlockClient(int fd, WorkerAddress addr) : fd_(fd), addr_(std::move(addr)) {}
     ~BlockClient();
     int fd() const { return fd_; }
     const WorkerAddress& addr() const { return addr_; }
-    // send one request frame, receive one response frame (heartbeats skipped), check echoes, map error responses
+    // send one request frame and read its answer
     Err rpc(const Protocol& req, const std::string& header, Protocol* resp, std::string* resp_header, std::string* resp_data);
+    // the answer to `req`: prefix and header (heartbeats skipped), the payload into *data (resized in place), the echo check, and an
+    // error status decoded into the worker's Err
+    Err recv_answer(const Protocol& req, Protocol* resp, std::string* header, std::string* data);
+    // request frame -> the end of `out`: prefix + header; the caller sends the data_len payload bytes behind it
+    static void append_frame(const Protocol& req, const std::string& header, std::string* out, int32_t data_len = 0);
     Err open_block(const ClientConf& conf, const ExtendedBlock& b, int64_t off, int64_t len, int64_t req_id, int32_t seq_id, bool short_circuit,
                    int64_t chunk_size, BlockReadResponse* out, bool accept_arena = false);
     Err read_commit(const ExtendedBlock& b, int64_t req_id, int32_t seq_id);
@@ -102,8 +112,7 @@ class BlockClient {
     // echo / status checked -- before the next request goes out on this connection (drain_pending), also after a trip through the pool.
     Err read_commit_deferred(const ExtendedBlock& b, int64_t req_id, int32_t seq_id);
     // Short-circuit Opens of several blocks in ONE write, then their answers in order (after those of the deferred Completes still
-    // owed); Completes (seq_id 1) of several blocks in one write, deferred.  Same messages and request ids as one call per block.  Any error leaves
-    // the connection broken: answers behind the failed one may still be on the wire.
+    // owed); Completes (seq_id 1) of several blocks in one write, deferred.  Same messages and request ids as one call per block.
     struct OpenReq {
         const ExtendedBlock* b;
         int64_t off, req_id;
@@ -117,12 +126,11 @@ class BlockClient {
     // data frames, and the Complete's answer stays pending like a deferred Complete.  Same messages, same order, two round trips less.
     Err send_block_read_pipeline(const ClientConf& conf, const ExtendedBlock& b, int64_t off, int64_t req_id, int64_t chunk_size, int64_t n_running,
                                  BlockReadResponse* open_resp);
-    Err send_request(const Protocol& req, const std::string& header);
-    Err recv_response_head(Protocol* resp, std::string* resp_header);  // prefix + header; payload left on the socket
     bool broken = false;
     int64_t idle_since_ms = 0;  // set when the connection goes back to the pool (BlockClient::uptime, block_client.rs:47,80-86)
 
    private:
+    Err send_request(const Protocol& req, const std::string& header);
     int fd_;
     WorkerAddress addr_;
     std::vector<Protocol> pending_;  // requests whose responses are still on the wire (deferred Completes)
@@ -139,6 +147,8 @@ class FsContext {
     // is dropped when acquire meets it
     Err acquire_read(const WorkerAddress& addr, std::unique_ptr<BlockClient>* out);
     void release(std::unique_ptr<BlockClient> c);
+    // keeps *conn when it goes to `addr` and is not broken; otherwise releases it and acquires a connection to `addr`
+    Err connection_to(const WorkerAddress& addr, std::unique_ptr<BlockClient>* conn);
     bool is_local_worker(const WorkerAddress& addr) const { return addr.hostname == conf.client.hostname; }
     int64_t read_chunk_size() const { return conf.client.read_chunk_size; }
     // fs_context.rs:83-86,182-205: workers excluded for failed_worker_ttl.  As in the reference only the write path adds to the list;

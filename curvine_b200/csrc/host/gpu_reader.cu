@@ -425,12 +425,8 @@ template <typename F>
 static Err for_each_replica(FsContext* ctx, const LocatedBlock& lb, std::unique_ptr<BlockClient>* conn, F fn) {
     Err last = ctx->no_available_worker(lb.locs);
     for (const WorkerAddress& loc : lb.locs) {
-        if (!*conn || !((*conn)->addr() == loc) || (*conn)->broken) {
-            if (*conn) ctx->release(std::move(*conn));
-            last = ctx->acquire_read(loc, conn);
-            if (last) continue;
-        }
-        last = fn(conn->get());
+        last = ctx->connection_to(loc, conn);
+        if (!last) last = fn(conn->get());
         if (!last) return Err::ok();
     }
     return last;
@@ -893,10 +889,7 @@ struct GpuFsReader::Call {
             if (!(jobs[j].lb->locs[0] == a)) return false;
             reqs.push_back(BlockClient::OpenReq{&jobs[j].lb->block, jobs[j].block_off, new_req_id()});
         }
-        if (!*conn || !((*conn)->addr() == a) || (*conn)->broken) {
-            if (*conn) r.ctx_->release(std::move(*conn));
-            if (r.ctx_->acquire_read(a, conn)) return false;
-        }
+        if (r.ctx_->connection_to(a, conn)) return false;
         if ((*conn)->open_blocks(r.ctx_->conf.client, reqs, r.ctx_->read_chunk_size(), r.ctx_->conf.b200.arena, resps)) return false;
         for (const BlockReadResponse& x : *resps)
             if (!x.has_path) {

@@ -48,6 +48,12 @@ Err decode_protocol(const uint8_t in[kProtocolSize], Protocol* p) {
     return Err::ok();
 }
 
+Protocol request_proto(int8_t code, int8_t req_status, int64_t req_id, int32_t seq_id) {
+    Protocol p;
+    p.code = code, p.req_status = req_status, p.resp_status = kRespUndefined, p.req_id = req_id, p.seq_id = seq_id;
+    return p;
+}
+
 // ---- proto2 as prost 0.11 writes it: required fields always present, in field order
 static void put_varint(std::string* s, uint64_t v) {
     while (v >= 0x80) {

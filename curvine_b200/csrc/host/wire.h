@@ -51,6 +51,8 @@ struct Protocol {
 void encode_protocol(const Protocol& p, uint8_t out[kProtocolSize]);
 // rpc_message.rs:326-338: rejects data_len < 0 and > 16 MiB
 Err decode_protocol(const uint8_t in[kProtocolSize], Protocol* p);
+// a request's prefix fields; header_len and data_len are set where the frame is encoded
+Protocol request_proto(int8_t code, int8_t req_status, int64_t req_id, int32_t seq_id);
 
 struct BlockReadRequest {  // worker.proto:38-47
     int64_t id = 0, off = 0, len = 0;

@@ -31,12 +31,6 @@ Err FsWriter::create(FsContext* ctx, const std::string& path, int64_t inode_id, 
     return Err::ok();
 }
 
-static Protocol write_req(int8_t status, int64_t req_id, int32_t seq_id) {
-    Protocol p;
-    p.code = kCodeWriteBlock, p.req_status = status, p.resp_status = kRespUndefined, p.req_id = req_id, p.seq_id = seq_id;
-    return p;
-}
-
 Err FsWriter::open_block() {
     LocatedBlock lb;
     CV_RETURN_IF_ERR(create_block_id(fb_.status.id, static_cast<int64_t>(fb_.block_locs.size()), &lb.block.id));
@@ -48,7 +42,7 @@ Err FsWriter::open_block() {
     r.off = 0, r.block_size = block_size_, r.chunk_size = static_cast<int32_t>(chunk_size_), r.client_name = "curvine-b200";
     Protocol resp;
     std::string rh, rd;
-    CV_RETURN_IF_ERR(client_->rpc(write_req(kReqOpen, req_id_, 0), r.encode(), &resp, &rh, &rd));
+    CV_RETURN_IF_ERR(client_->rpc(request_proto(kCodeWriteBlock, kReqOpen, req_id_, 0), r.encode(), &resp, &rh, &rd));
     BlockWriteResponse wr;
     CV_RETURN_IF_ERR(BlockWriteResponse::decode(reinterpret_cast<const uint8_t*>(rh.data()), rh.size(), &wr));
     if (wr.block_size != block_size_)
@@ -68,7 +62,7 @@ Err FsWriter::commit_block(bool cancel) {
     r.off = block_pos_, r.block_size = block_size_, r.client_name = "curvine-b200";
     Protocol resp;
     std::string rh, rd;
-    CV_RETURN_IF_ERR(client_->rpc(write_req(cancel ? kReqCancel : kReqComplete, req_id_, ++seq_), r.encode(), &resp, &rh, &rd));
+    CV_RETURN_IF_ERR(client_->rpc(request_proto(kCodeWriteBlock, cancel ? kReqCancel : kReqComplete, req_id_, ++seq_), r.encode(), &resp, &rh, &rd));
     block_open_ = false;
     if (cancel) fb_.block_locs.pop_back();
     return Err::ok();
@@ -76,25 +70,17 @@ Err FsWriter::commit_block(bool cancel) {
 
 // one Running request carrying `n` payload bytes, then its (empty) success response
 Err FsWriter::send_running(const uint8_t* payload, int64_t n) {
-    Protocol p = write_req(kReqRunning, req_id_, ++seq_);
-    p.header_len = 0, p.data_len = static_cast<int32_t>(n);
-    uint8_t prefix[kProtocolSize];
-    encode_protocol(p, prefix);
-    Err e = send_all(client_->fd(), prefix, kProtocolSize);
+    const Protocol req = request_proto(kCodeWriteBlock, kReqRunning, req_id_, ++seq_);
+    std::string prefix;
+    BlockClient::append_frame(req, std::string(), &prefix, static_cast<int32_t>(n));
+    Err e = send_all(client_->fd(), prefix.data(), prefix.size());
     if (!e) e = send_all(client_->fd(), payload, static_cast<size_t>(n));
+    if (e) client_->broken = true;
     Protocol resp;
-    std::string rh;
-    if (!e) e = client_->recv_response_head(&resp, &rh);
-    if (e) {
-        client_->broken = true;
-        ctx_->add_failed_worker(worker_);
-        return e;
-    }
-    std::string body(static_cast<size_t>(resp.data_len), '\0');
-    if (resp.data_len && (e = recv_exact(client_->fd(), &body[0], body.size()))) return e;
-    if (resp.req_id != req_id_ || resp.seq_id != seq_) return Err::common("response mismatch");
-    if (!resp.is_success()) return decode_error_body(reinterpret_cast<const uint8_t*>(body.data()), body.size());
-    return Err::ok();
+    std::string rh, rd;
+    if (!e) e = client_->recv_answer(req, &resp, &rh, &rd);
+    if (e && client_->broken) ctx_->add_failed_worker(worker_);  // a well-formed error answer leaves the worker off the list
+    return e;
 }
 
 Err FsWriter::write(const uint8_t* buf, int64_t n) {
@@ -125,15 +111,10 @@ Err FsWriter::write_device(const void* d_src, int64_t n, void* stream) {
                                              req_id_, seq_ + 1, stream, &packed_, &crc32));
         // all Running frames of this range in one write, then their responses (the worker serves them in order)
         Err e = send_all(client_->fd(), packed_.wire, wire_bytes);
-        for (uint32_t f = 0; f < nf && !e; f++) {
-            Protocol resp;
-            std::string rh;
-            e = client_->recv_response_head(&resp, &rh);
-            std::string body(e ? 0 : static_cast<size_t>(resp.data_len), '\0');
-            if (!e && resp.data_len) e = recv_exact(client_->fd(), &body[0], body.size());
-            if (!e && (resp.req_id != req_id_ || resp.seq_id != seq_ + 1 + static_cast<int32_t>(f))) e = Err::common("response mismatch");
-            if (!e && !resp.is_success()) e = decode_error_body(reinterpret_cast<const uint8_t*>(body.data()), body.size());
-        }
+        Protocol resp;
+        std::string rh, rd;
+        for (uint32_t f = 0; f < nf && !e; f++)
+            e = client_->recv_answer(request_proto(kCodeWriteBlock, kReqRunning, req_id_, seq_ + 1 + static_cast<int32_t>(f)), &resp, &rh, &rd);
         if (e) {
             client_->broken = true;
             return e;

@@ -4,7 +4,8 @@ handler errors into error RESPONSES (block_handler.rs:57-60).  Here both ends of
   * the WORKER is fed malformed, truncated and random frames over raw sockets: it must answer with an error frame or drop the connection,
     never crash, never allocate what a length field claims, and keep serving well-behaved clients;
   * the CLIENT (host reader, framed path) talks to a worker that lies: absurd lengths, wrong echoes, truncated payloads, payloads longer
-    than asked for, random bytes, silence.  Every call must come back with an error (or the correct bytes), within its timeout.
+    than asked for, random bytes, silence.  Every call must come back with an error (or the correct bytes), within its timeout.  The host
+    writer meets wrong echoes, an error answer and a cut-off answer, and must not pool a connection whose stream is out of step.
 
 tools/sanitize_host.sh runs this file under ASan+UBSan."""
 import os
@@ -133,6 +134,9 @@ class _LyingWorker:
                 header = self._rx(c, hlen)
                 self._rx(c, total - 18 - hlen)
                 st = pre[9] & 0x0f
+                if st == W.REQ_OPEN and pre[8] == W.RPC_CODE_WRITE_BLOCK:  # a writer's Open: the block size it asked for
+                    c.sendall(self._reply(pre, header=W.BlockWriteResponse(block_size=W.BlockWriteRequest.decode(header).block_size, storage_type=0).encode()))
+                    continue
                 if st == W.REQ_OPEN:
                     req = W.BlockReadRequest.decode(header)
                     pos, chunk = req.off, req.chunk_size
@@ -165,6 +169,10 @@ class _LyingWorker:
                     c.sendall(self._reply(pre, data=data, seq_id=-1))
                 elif m == "truncated_payload":
                     c.sendall(self._reply(pre, data=data)[:22 + len(data) // 2])
+                    c.close()
+                    return
+                elif m == "truncated_then_hang_up":  # a payload announced, half of it sent
+                    c.sendall(self._reply(pre, data=b"\0" * 64)[:22 + 32])
                     c.close()
                     return
                 elif m == "longer_than_chunk":
@@ -224,6 +232,26 @@ def test_client_survives_a_lying_worker(mode):
     finally:
         lw.close()
     assert time.time() - t0 < 30, "a lying worker must not stall the client beyond its timeouts"
+
+
+@pytest.mark.parametrize("mode", ["wrong_seq_id", "wrong_req_id", "error_response", "truncated_then_hang_up"])
+def test_writer_survives_a_lying_worker(mode):
+    """The answer to a host write's Running lies.  write() fails, and the connection goes back to the pool only when its stream is still
+    in step: after a well-formed error answer, never after a wrong echo or a cut-off payload."""
+    lw = _LyingWorker(b"", mode, random.Random(99))  # Running answers carry no payload, as a worker's do
+    try:
+        with F.CurvineFileSystem(F.client_conf(extra_client='conn_timeout_ms = 1000\ndata_timeout_ms = 1000\nrpc_timeout_ms = 1000\n')) as fs:
+            w = fs.create("/lie_w", 4802, 1 << 20, lw.port)
+            with pytest.raises(F.FsError):
+                w.write(b"x" * 1000)
+            try:
+                w.complete()
+            except F.FsError:
+                if mode != "truncated_then_hang_up":  # only a worker that hung up cannot answer the Complete
+                    raise
+            assert fs.pool_stats()["idle"] == (1 if mode == "error_response" else 0)
+    finally:
+        lw.close()
 
 
 def test_conf_and_manifest_parsers_survive_garbage():
